@@ -383,13 +383,20 @@ const FastCfg kMma32V2[] = {
     MmaInst2<32, 1, 2, 512, 128, 3, 2, 9>::cfg(),  // h: g + seed
 };
 #endif  // TPE_LAB
-// P = 32 at config 2 on H100 (CUDA events, g(x) launch): 256-thread CTAs with two kernel groups in flight per
-// warp, a 2-stage ring and 3 CTAs per SM take 1.38 ms, against 1.43-1.44 ms for 512-thread CTAs with a 3-stage
-// ring (KG = 1, 2) and for KG = 4.  The other widths keep the tilings chosen on another GPU.
+// Tilings measured on an H100 SXM (400 W power limit, 1980 MHz max SM clock), CUDA events around the g(x)
+// launch, 100k kernels (tools/tune_mma.py).  M = 2 issues mma.m16n8k8 (twice the m8n8k4 rate on H100), M = 1
+// issues m8n8k4.  With two candidate groups per warp a thread needs 120-200 registers, so the big path runs
+// 16 warps per SM (8 for P = 64); the probe (tools/probe_dmma2.cu) shows that 8 warps with one m16n8k8 chain
+// each already saturate the pipe.  4096 candidates:
+//   P = 16: 1.18 ms (m8n8k4: 1.27)   P = 32: 1.14 ms (m8n8k4: 1.41)   P = 64: 1.77 ms (m8n8k4: 2.15)
+//   P = 8: m8n8k4 stays faster: 1.151-1.154 ms against 1.190 ms for the best m16n8k8 tiling in three alternated
+//   pairs of runs (the means of one tiling spread by 0.003 ms, the gap is 0.037 ms).
+// Small path (one ask of 24 candidates): m8n8k4 stays (the best m16n8k8 tiling is no faster at P = 64 and
+// 14-30 % slower at the other widths).
 //                                   PB M KG  NT   TK ST MINB
 const FastCfg kMmaBig[] = {
-    MmaInst<8, 1, 4, 256, 512, 3, 2>::cfg(), MmaInst<16, 1, 4, 256, 256, 3, 2>::cfg(),
-    MmaInst<32, 1, 2, 256, 128, 2, 3>::cfg(), MmaInst<64, 1, 2, 256, 64, 3, 1>::cfg(),
+    MmaInst<8, 1, 4, 256, 512, 3, 2>::cfg(), MmaInst<16, 2, 2, 256, 256, 3, 2>::cfg(),
+    MmaInst<32, 2, 1, 256, 128, 2, 2>::cfg(), MmaInst<64, 2, 2, 256, 64, 3, 1>::cfg(),
 };
 const FastCfg kMmaSmall[] = {
     MmaInst<8, 1, 4, 64, 512, 3, 4>::cfg(), MmaInst<16, 1, 4, 64, 256, 3, 4>::cfg(),
@@ -402,11 +409,53 @@ const FastCfg kMma32Variants[] = {
     MmaInst<32, 1, 2, 512, 128, 3, 2>::cfg(), MmaInst<32, 1, 2, 512, 128, 3, 2, 1>::cfg(),
     MmaInst<32, 1, 2, 512, 128, 3, 2, 2>::cfg(), MmaInst<32, 1, 4, 256, 128, 3, 2, 1>::cfg(),
 };
+// Tilings for every width, big and small path, selected by TPE_MMA_LAB=<index> when the width matches
+// (tools/tune_mma.py); DBG = 1 / 2 time the mma + TMA floor and the classification + far tier alone, DBG = 3
+// starts the accumulator at ckk - base (no per-term DADD before the classification).
+//                                   PB M KG  NT   TK ST MINB DBG
+const FastCfg kMmaLab[] = {
+    MmaInst<32, 1, 2, 256, 128, 2, 3, 1>::cfg(),  //  0
+    MmaInst<32, 1, 2, 256, 128, 2, 3, 2>::cfg(),  //  1
+    MmaInst<32, 2, 1, 256, 128, 2, 2>::cfg(),     //  2
+    MmaInst<32, 2, 2, 256, 128, 2, 2>::cfg(),     //  3
+    MmaInst<32, 2, 1, 256, 128, 2, 3>::cfg(),     //  4
+    MmaInst<32, 2, 2, 256, 128, 2, 2, 1>::cfg(),  //  5
+    MmaInst<32, 2, 2, 256, 128, 2, 2, 2>::cfg(),  //  6
+    MmaInst<32, 2, 1, 256, 128, 2, 2, 1>::cfg(),  //  7
+    MmaInst<32, 2, 1, 256, 128, 2, 2, 2>::cfg(),  //  8
+    MmaInst<32, 2, 1, 512, 128, 3, 1>::cfg(),     //  9
+    MmaInst<32, 2, 2, 512, 128, 2, 1>::cfg(),     // 10
+    MmaInst<32, 2, 1, 128, 128, 2, 4>::cfg(),     // 11
+    MmaInst<32, 2, 2, 64, 128, 3, 4>::cfg(),      // 12  small
+    MmaInst<32, 2, 1, 64, 128, 3, 4>::cfg(),      // 13  small
+    MmaInst<32, 2, 4, 64, 128, 3, 2>::cfg(),      // 14  small
+    MmaInst<8, 2, 2, 256, 512, 3, 2>::cfg(),      // 15
+    MmaInst<8, 2, 4, 256, 512, 3, 2>::cfg(),      // 16
+    MmaInst<8, 2, 2, 256, 512, 3, 3>::cfg(),      // 17
+    MmaInst<8, 2, 2, 64, 512, 3, 4>::cfg(),       // 18  small
+    MmaInst<8, 2, 4, 64, 512, 3, 4>::cfg(),       // 19  small
+    MmaInst<16, 2, 2, 256, 256, 3, 2>::cfg(),     // 20
+    MmaInst<16, 2, 4, 256, 256, 3, 2>::cfg(),     // 21
+    MmaInst<16, 2, 2, 256, 256, 2, 3>::cfg(),     // 22
+    MmaInst<16, 2, 2, 64, 256, 3, 4>::cfg(),      // 23  small
+    MmaInst<16, 2, 4, 64, 256, 3, 4>::cfg(),      // 24  small
+    MmaInst<64, 2, 1, 256, 64, 3, 1>::cfg(),      // 25
+    MmaInst<64, 2, 2, 256, 64, 3, 1>::cfg(),      // 26
+    MmaInst<64, 2, 1, 256, 64, 2, 2>::cfg(),      // 27
+    MmaInst<64, 2, 1, 64, 64, 3, 3>::cfg(),       // 28  small
+    MmaInst<64, 2, 2, 64, 64, 3, 3>::cfg(),       // 29  small
+    MmaInst<32, 2, 1, 256, 128, 2, 2, 3>::cfg(),  // 30  accumulator initialised with ckk - base
+};
+constexpr int kMmaLabN = sizeof(kMmaLab) / sizeof(kMmaLab[0]);
 #endif  // TPE_LAB
 
 const FastCfg* pick_mma(int pb, int64_t Ct) {
   const bool small = Ct <= 64;
 #ifdef TPE_LAB
+  if (const char* v = getenv("TPE_MMA_LAB")) {
+    const int i = atoi(v);
+    if (i >= 0 && i < kMmaLabN && kMmaLab[i].pb == pb) return &kMmaLab[i];
+  }
   if (pb == 32 && !small) {
     const char* v = getenv("TPE_MMA_VARIANT");
     if (v && v[0] >= '0' && v[0] <= '7') return &kMma32Variants[v[0] - '0'];

@@ -595,7 +595,8 @@ __global__ void k_tab_pad(double2* __restrict__ tabp, double* __restrict__ tabc,
 // Fragment-major layout of the CONST table for the tensor-core kernel (k_logpdf_mma): kernels in
 // groups of 8, inside a group the order in which the 32 lanes of a warp read their B fragments of
 // mma.m8n8k4 (lane = 4 * (k % 8) + slot % 4 holds B[row = slot % 4][col = k % 8] of k-step slot / 4),
-// two k-steps interleaved so that one LDS.128 per lane fetches both.
+// two k-steps interleaved so that one LDS.128 per lane fetches both.  The pair is also exactly the B fragment
+// {b0, b1} of one mma.m16n8k8 over the 8 slots of both k-steps.
 __host__ __device__ __forceinline__ int64_t mma_tab_index(int64_t k, int slot, int pb) {
   const int i = slot >> 2;
   const int lane = (int)(k & 7) * 4 + (slot & 3);
@@ -1562,14 +1563,18 @@ struct LseTier {
   // N terms at once: the classification and the far-tier exps of all of them are independent
   // (pipelined through the fp64 / SFU / fp32 pipes), one vote decides whether any lane has a near
   // term at all -- rare once base has converged (< 1 % of the terms are near).
-  template <int N, bool EXACT>
-  __device__ __forceinline__ void push_batch(const double (&L)[N], float skip, float tnear) {
+  // SHIFTED (timing experiment): L holds L - sh, with sh = base (or 0 while base = -inf), so the classification
+  // needs no DADD and L is rebuilt only for the parked terms.
+  template <int N, bool EXACT, bool SHIFTED = false>
+  __device__ __forceinline__ void push_batch(const double (&L)[N], float skip, float tnear, double sh = 0.0) {
     bool near[N];
     bool any = false;
     float add = 0.0f;
+    const bool cold = SHIFTED && base == -INFINITY;
 #pragma unroll
     for (int i = 0; i < N; ++i) {
-      const float df = __double2float_rn(L[i] - base);  // base = -inf -> +inf -> near
+      const float df = SHIFTED ? (cold ? INFINITY : __double2float_rn(L[i]))
+                               : __double2float_rn(L[i] - base);  // base = -inf -> +inf -> near
       near[i] = df > -tnear;
       const bool far = !near[i] && df > -skip;
       const float e = ex2_approx(df * 1.44269504f);
@@ -1582,7 +1587,7 @@ struct LseTier {
       // enough by construction) even if a flush below raises base
 #pragma unroll
       for (int i = 0; i < N; ++i)
-        if (__any_sync(0xffffffffu, near[i])) park(L[i], near[i]);
+        if (__any_sync(0xffffffffu, near[i])) park(SHIFTED ? L[i] + sh : L[i], near[i]);
     }
   }
 };
@@ -1594,15 +1599,18 @@ struct LseTier {
 //   a_cp = (x_cp - ctr_p) / sigma_p,  b_kp = (mu_kp - ctr_p) / sigma_p,
 //   L[c,k] = cst_k - |a_c - b_k|^2 / 2 = (cst_k - |b_k|^2 / 2) + a_c . b_k - |a_c|^2 / 2,
 // i.e. ONE fma per cell instead of two, and the a . b part is a [C x P] x [P x K] fp64 GEMM: it runs
-// on the fp64 tensor-core path (mma.sync m8n8k4, SASS DMMA.8x8x4 -- on H100 the same rate as DFMA, but
-// 256 fma per warp instruction with the operands shared in registers, so neither the
-// issue slots nor the shared-memory pipe limit it).  The accumulator fragment is initialised with
+// on the fp64 tensor-core path with the operands shared in registers, so neither the issue slots nor the
+// shared-memory pipe limit it.  With M even a warp owns pairs of candidate groups and issues mma.sync
+// m16n8k8 (SASS DMMA.16x8x8, 1024 fma per warp instruction, twice the DFMA rate on H100); with M = 1 it
+// issues m8n8k4 (DMMA.8x8x4, 256 fma, the DFMA rate on H100), which still wins for a single small ask.
+// Both read the same registers and table: one m16n8k8 does the work of four m8n8k4 (two k-steps x two
+// candidate groups), only the order of the roundings inside one k8 step differs.  The accumulator fragment is initialised with
 // cst_k - |b_k|^2 / 2 (host side of the build), so L - ha_c falls out of the mma chain directly and
 // -|a_c|^2 / 2 is added once per candidate after the log-sum-exp (shift invariance).
 // Rounding: |a|, |b| <= rho = range / (2 sigma); the expanded form loses ~P * rho^2 * 2^-52 absolute
 // (8e-14 at config 2); the host falls back to k_logpdf_fast when that bound exceeds 5e-13.
 //
-//   rows of A = candidates (8 per mma, M groups per warp), columns of B = kernels (8 per mma);
+//   rows of A = candidates (8 per group, M groups per warp), columns of B = kernels (8 per mma);
 //   lane (g = lane / 4, q = lane % 4) holds C[candidate g][kernels 2q, 2q + 1]: it owns one
 //   log-sum-exp state per candidate group and the 4 lanes of a candidate are merged at the end.
 //   tabm: fragment-major table (mma_tab_index), ckk: per-kernel constants (-inf padded to 8).
@@ -1612,15 +1620,26 @@ __device__ __forceinline__ void dmma_8x8x4(double& d0, double& d1, double a, dou
                : "+d"(d0), "+d"(d1)
                : "d"(a), "d"(b));
 }
-// KG kernel groups (8 kernels each) are in flight per warp: KG * M independent mma chains, which is
-// what keeps the DMMA pipe fed (a chain of 8 dependent DMMAs alone cannot hide the DMMA latency).
+// m16n8k8 (SASS DMMA.16x8x8, twice the DFMA rate on H100): rows g and g + 8 of A are two candidate groups,
+// a0..a3 = A[g][q], A[g + 8][q], A[g][q + 4], A[g + 8][q + 4]; b0, b1 = B[q][g], B[q + 4][g];
+// {d0, d1} = C[g][2q, 2q + 1], {d2, d3} = C[g + 8][2q, 2q + 1] -- the m8n8k4 fragments of two k-steps and
+// two candidate groups, so the table and the A registers are the same as for m8n8k4.
+__device__ __forceinline__ void dmma_16x8x8(double& d0, double& d1, double& d2, double& d3, double a0, double a1,
+                                            double a2, double a3, double b0, double b1) {
+  asm volatile("mma.sync.aligned.m16n8k8.row.col.f64.f64.f64.f64 {%0,%1,%2,%3}, {%4,%5,%6,%7}, {%8,%9}, {%0,%1,%2,%3};"
+               : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3)
+               : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
+}
+// KG kernel groups (8 kernels each) are in flight per warp: KG * M independent m8n8k4 chains (M = 1), or
+// KG * M / 2 m16n8k8 chains (M even, two candidate groups per instruction), which is what keeps the DMMA
+// pipe fed (one chain of dependent DMMAs alone cannot hide the DMMA latency).
 template <int PB, int M, int KG, int NT, int TK, int ST, int MINB, int DBG = 0>
 __global__ void __launch_bounds__(NT, MINB)
 k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, int64_t Kfp,
              const double2* __restrict__ colprm, const double* __restrict__ xT, int64_t ct_stride, int64_t kps,
              double lse_skip, double2* __restrict__ part, unsigned long long* __restrict__ gmax,
              double lse_near) {
-  static_assert(PB % 8 == 0 && TK % (8 * KG) == 0, "bad tiling");
+  static_assert(PB % 8 == 0 && TK % (8 * KG) == 0 && (M == 1 || M % 2 == 0), "bad tiling");
   constexpr int NI = PB / 4;        // k-steps of the mma chain
   constexpr int CW = 8 * M;         // candidates per warp
   extern __shared__ __align__(128) unsigned char smem_raw[];
@@ -1712,6 +1731,9 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
       }
       const double2* fb = reinterpret_cast<const double2*>(tile + (size_t)kg * 8 * PB) + lane;
       double d0[KG][M], d1[KG][M];
+      double sh[M];  // DBG = 3 (timing experiment): the accumulator starts at ckk - base
+#pragma unroll
+      for (int m = 0; m < M; ++m) sh[m] = (DBG == 3 && acc[m].base != -INFINITY) ? acc[m].base : 0.0;
 #pragma unroll
       for (int u = 0; u < KG; ++u) {
         const double2 cc = reinterpret_cast<const double2*>(ctile + (kg + u) * 8)[q];
@@ -1719,6 +1741,10 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
         for (int m = 0; m < M; ++m) {
           d0[u][m] = cc.x;
           d1[u][m] = cc.y;
+          if constexpr (DBG == 3) {
+            d0[u][m] -= sh[m];
+            d1[u][m] -= sh[m];
+          }
         }
       }
       double2 v[2][KG];
@@ -1730,14 +1756,19 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
 #pragma unroll
           for (int u = 0; u < KG; ++u) v[(i2 + 1) & 1][u] = fb[u * (4 * PB) + (i2 + 1) * 32];
         }
+        if constexpr (M % 2 == 0) {
 #pragma unroll
-        for (int u = 0; u < KG; ++u)
+          for (int u = 0; u < KG; ++u)
 #pragma unroll
-          for (int m = 0; m < M; ++m) dmma_8x8x4(d0[u][m], d1[u][m], a[m][2 * i2], v[i2 & 1][u].x);
+            for (int m = 0; m < M; m += 2)
+              dmma_16x8x8(d0[u][m], d1[u][m], d0[u][m + 1], d1[u][m + 1], a[m][2 * i2], a[m + 1][2 * i2],
+                          a[m][2 * i2 + 1], a[m + 1][2 * i2 + 1], v[i2 & 1][u].x, v[i2 & 1][u].y);
+        } else {
 #pragma unroll
-        for (int u = 0; u < KG; ++u)
+          for (int u = 0; u < KG; ++u) dmma_8x8x4(d0[u][0], d1[u][0], a[0][2 * i2], v[i2 & 1][u].x);
 #pragma unroll
-          for (int m = 0; m < M; ++m) dmma_8x8x4(d0[u][m], d1[u][m], a[m][2 * i2 + 1], v[i2 & 1][u].y);
+          for (int u = 0; u < KG; ++u) dmma_8x8x4(d0[u][0], d1[u][0], a[0][2 * i2 + 1], v[i2 & 1][u].y);
+        }
       }
 #pragma unroll
       for (int m = 0; m < M; ++m) {
@@ -1752,6 +1783,8 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
           for (int u = 0; u < 2 * KG; ++u) acc[m].fsum += vals[u];
         } else if constexpr (DBG == 2) {  // timing experiment: classification + far tier only
           acc[m].template push_batch<2 * KG, false>(vals, lim_skip, lim_near);
+        } else if constexpr (DBG == 3) {
+          acc[m].template push_batch<2 * KG, true, true>(vals, lim_skip, lim_near, sh[m]);
         } else {
           acc[m].template push_batch<2 * KG, true>(vals, lim_skip, lim_near);
         }
