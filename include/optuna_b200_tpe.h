@@ -35,7 +35,8 @@ extern "C" {
 /* 4: + tpe_sample_and_select_async / tpe_collect */
 /* 5: + tpe_suggest_univariate_batch_async / tpe_collect_univariate */
 /* 6: + tpe_set_kernel_shard / tpe_sample_and_partial / tpe_finish_from_partials */
-#define TPE_ABI_VERSION 6
+/* 7: + tpe_hypervolume_history */
+#define TPE_ABI_VERSION 7
 
 enum {
   TPE_OK = 0,
@@ -253,6 +254,16 @@ int tpe_get_split(tpe_ctx* ctx, int64_t* below_rows, int64_t* above_rows);
 int tpe_get_mixture(tpe_ctx* ctx, int which, double* weights, double* mu, double* sigma);
 /* MOTPE: raw hypervolume weights of ALL below trials (length n_below_all) of the last tpe_build. */
 int tpe_get_mo_weights(tpe_ctx* ctx, double* weights);
+
+/* ---- analysis ------------------------------------------------------------------------------ */
+/* Hypervolume history of a multi-objective study (replaces _get_hypervolume_history_info,
+ * optuna/visualization/_hypervolume_history.py:83-138).  values [n, n_objectives]: objective values of the
+ * COMPLETE trials in trial order, multiplied by +1 (minimise) or -1 (maximise); ref [n_objectives]: the
+ * reference point with the same signs; feasible [n]: 0 = a constraint is violated (NULL: all feasible).
+ * out [n]: the hypervolume after each trial.  2 <= n_objectives <= 16; NaN in values or ref is
+ * TPE_E_INVALID.  Uses its own device memory and leaves the context's history and suggestion state alone. */
+int tpe_hypervolume_history(tpe_ctx* ctx, const double* values, const uint8_t* feasible, int64_t n,
+                            int32_t n_objectives, const double* ref, double* out);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

@@ -19,6 +19,7 @@
 #include "../../include/optuna_b200_tpe.h"
 #include "tpe_kernels.cuh"
 #include "tpe_motpe_kernels.cuh"
+#include "tpe_hvhist.cuh"
 #include "tpe_uni.cuh"
 #include "tpe_mixed.cuh"
 #include "tpe_tcscreen.cuh"
@@ -1775,6 +1776,123 @@ static int uni_batch_staged(tpe_ctx* ctx, const tpe_cfg* cfg, const int32_t* col
   return TPE_OK;
 }
 
+// ---- hypervolume history (tpe_hvhist.cuh) -------------------------------------------------------
+// Device memory of one tpe_hypervolume_history call, released when it returns: nothing a suggestion reads is touched.
+struct HhScratch {
+  DevBuf v, feas, ref, elig, added, list, rank, K, death, incl, cnt, off, clip, keep, surv, m, soff, arena, hv, cum, out;
+  ~HhScratch() {
+    for (DevBuf* b : {&v, &feas, &ref, &elig, &added, &list, &rank, &K, &death, &incl, &cnt, &off, &clip, &keep, &surv, &m,
+                      &soff, &arena, &hv, &cum, &out})
+      b->release();
+  }
+};
+// Memory bounds per pass: the clipped fronts of one chunk of added trials (clip and surv each) and the hypervolume
+// scratch of one launch.  A single trial that needs more gets a chunk of its own, sized for it.
+constexpr size_t kHhClipDoubles = (size_t)1 << 25;
+constexpr size_t kHhHvDoubles = (size_t)1 << 26;
+
+int hv_history_run(tpe_ctx* ctx, const double* values, const uint8_t* feasible, int n, int M, const double* ref,
+                   double* out) {
+  cudaStream_t st = ctx->stream;
+  HhScratch s;
+  const size_t vb = (size_t)n * M * 8;
+  CU(s.v.ensure(vb));
+  CU(s.ref.ensure((size_t)M * 8));
+  CU(cudaMemcpyAsync(s.v.p, values, vb, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.ref.p, ref, (size_t)M * 8, cudaMemcpyHostToDevice, st));
+  if (feasible) {
+    CU(s.feas.ensure((size_t)n));
+    CU(cudaMemcpyAsync(s.feas.p, feasible, (size_t)n, cudaMemcpyHostToDevice, st));
+  }
+  for (DevBuf* b : {&s.elig, &s.added}) CU(b->ensure((size_t)n));
+  for (DevBuf* b : {&s.list, &s.rank}) CU(b->ensure((size_t)n * 4));
+  CU(s.K.ensure(4));
+  const double* v = s.v.as<double>();
+  const double* dref = s.ref.as<double>();
+  const int nb = (n + kHhThreads - 1) / kHhThreads;
+  k_hh_eligible<<<nb, kHhThreads, 0, st>>>(v, feasible ? s.feas.as<uint8_t>() : nullptr, n, M, dref,
+                                           s.elig.as<uint8_t>());
+  k_hh_added<<<nb, kHhThreads, hh_added_smem(M), st>>>(v, n, M, s.elig.as<uint8_t>(), s.added.as<uint8_t>());
+  k_hh_compact<<<1, 1024, 0, st>>>(s.added.as<uint8_t>(), n, s.list.as<int32_t>(), s.rank.as<int32_t>(),
+                                   s.K.as<int32_t>());
+  CU(cudaGetLastError());
+  int K = 0;
+  CU(cudaMemcpyAsync(&K, s.K.p, 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (K > 0) {
+    const int kb = (K + kHhThreads - 1) / kHhThreads;
+    for (DevBuf* b : {&s.death, &s.cnt, &s.m}) CU(b->ensure((size_t)K * 4));
+    for (DevBuf* b : {&s.incl, &s.hv, &s.cum}) CU(b->ensure((size_t)K * 8));
+    k_hh_death<<<kb, kHhThreads, hh_added_smem(M), st>>>(v, n, M, s.list.as<int32_t>(), K, dref,
+                                                          s.death.as<int32_t>(), s.incl.as<double>());
+    k_hh_count<<<kb, kHhThreads, 0, st>>>(s.list.as<int32_t>(), s.death.as<int32_t>(), K, s.cnt.as<int32_t>());
+    CU(cudaGetLastError());
+    std::vector<int32_t> cnt((size_t)K), m((size_t)K);
+    CU(cudaMemcpyAsync(cnt.data(), s.cnt.p, (size_t)K * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    std::vector<int64_t> off((size_t)K + 1, 0), soff((size_t)K);
+    for (int p = 0; p < K; ++p) off[p + 1] = off[p] + cnt[p];
+    CU(s.off.ensure((size_t)(K + 1) * 8));
+    CU(s.soff.ensure((size_t)K * 8));
+    CU(cudaMemcpyAsync(s.off.p, off.data(), (size_t)(K + 1) * 8, cudaMemcpyHostToDevice, st));
+    // chunks [pa, pb) of added trials whose clipped fronts fit the bound, sized before any kernel reads them
+    std::vector<int> cuts{0};
+    size_t rows_max = 1;
+    while (cuts.back() < K) {
+      const int pa = cuts.back();
+      int pb = pa + 1;
+      while (pb < K && (size_t)(off[pb + 1] - off[pa]) * M <= kHhClipDoubles) ++pb;
+      rows_max = std::max(rows_max, (size_t)(off[pb] - off[pa]));
+      cuts.push_back(pb);
+    }
+    CU(s.clip.ensure(rows_max * M * 8));
+    CU(s.surv.ensure(rows_max * M * 8));
+    CU(s.keep.ensure(rows_max));
+    for (size_t c = 0; c + 1 < cuts.size(); ++c) {
+      const int pa = cuts[c], pb = cuts[c + 1];
+      k_hh_front<<<(pb - pa + 3) / 4, kHhThreads, 0, st>>>(v, M, s.list.as<int32_t>(), s.death.as<int32_t>(),
+                                                           s.cnt.as<int32_t>(), s.off.as<int64_t>(), pa, pb,
+                                                           s.clip.as<double>(), s.keep.as<uint8_t>(),
+                                                           s.surv.as<double>(), s.m.as<int32_t>());
+      CU(cudaGetLastError());
+      // (this wait also ends the previous chunk's hypervolume launches, so the arena may be reallocated below)
+      CU(cudaMemcpyAsync(m.data() + pa, s.m.as<int32_t>() + pa, (size_t)(pb - pa) * 4, cudaMemcpyDeviceToHost, st));
+      CU(cudaStreamSynchronize(st));
+      // launches [qa, qb) of this chunk whose hypervolume scratch fits the bound; soff is relative to each launch
+      std::vector<std::pair<int, int>> launches;
+      size_t need = 0, arena = 1;
+      int qa = pa;
+      for (int p = pa; p < pb; ++p) {
+        const size_t d = (hh_hv_scratch_doubles(m[p], M) + 1) & ~(size_t)1;
+        if (p > qa && need + d > kHhHvDoubles) {
+          launches.push_back({qa, p});
+          qa = p;
+          need = 0;
+        }
+        soff[p] = (int64_t)need;
+        need += d;
+        arena = std::max(arena, need);
+      }
+      launches.push_back({qa, pb});
+      CU(s.arena.ensure(arena * 8));
+      CU(cudaMemcpyAsync(s.soff.as<int64_t>() + pa, soff.data() + pa, (size_t)(pb - pa) * 8, cudaMemcpyHostToDevice, st));
+      for (auto& q : launches)
+        k_hh_hv<<<(q.second - q.first + 3) / 4, kHhThreads, 0, st>>>(
+            M, s.cnt.as<int32_t>(), s.off.as<int64_t>(), pa, q.first, q.second, s.surv.as<double>(),
+            s.m.as<int32_t>(), dref, s.soff.as<int64_t>() + pa, s.arena.as<double>(), s.hv.as<double>());
+      CU(cudaGetLastError());
+    }
+    k_hh_scan<<<1, 1, 0, st>>>(K, s.incl.as<double>(), s.hv.as<double>(), s.cum.as<double>());
+  }
+  CU(s.out.ensure((size_t)n * 8));
+  k_hh_fill<<<nb, kHhThreads, 0, st>>>(s.rank.as<int32_t>(), n, K > 0 ? s.cum.as<double>() : nullptr,
+                                       s.out.as<double>());
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out, s.out.p, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
 
 // =================================================================================================
 extern "C" {
@@ -2020,6 +2138,23 @@ int tpe_get_mo_weights(tpe_ctx* ctx, double* weights) {
   CU(cudaMemcpyAsync(weights, ctx->mo_w.p, (size_t)ctx->info.n_below_all * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CU(cudaStreamSynchronize(ctx->stream));
   return TPE_OK;
+}
+
+int tpe_hypervolume_history(tpe_ctx* ctx, const double* values, const uint8_t* feasible, int64_t n,
+                            int32_t n_objectives, const double* ref, double* out) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  const int M = n_objectives;
+  if (M < 2 || M > kMoMaxM) return fail(ctx, TPE_E_INVALID, "n_objectives must be in [2, %d]", kMoMaxM);
+  if (n < 0 || n >= (1ll << 31) - 4096) return fail(ctx, TPE_E_INVALID, "bad number of trials %lld", (long long)n);
+  if (!ref || (n > 0 && (!values || !out))) return fail(ctx, TPE_E_INVALID, "bad hypervolume history arguments");
+  for (int j = 0; j < M; ++j)
+    if (std::isnan(ref[j])) return fail(ctx, TPE_E_INVALID, "the reference point holds NaN");
+  for (int64_t q = 0; q < n * M; ++q)
+    if (std::isnan(values[q])) return fail(ctx, TPE_E_INVALID, "objective values hold NaN (trial %lld)", (long long)(q / M));
+  if (n == 0) return TPE_OK;
+  if (set_device(ctx, false)) return TPE_E_CUDA;
+  return hv_history_run(ctx, values, feasible, (int)n, M, ref, out);
 }
 
 int64_t tpe_history_size(tpe_ctx* ctx) { return ctx ? ctx->N : -1; }

@@ -361,6 +361,25 @@ class TPEEngine:
         self._check(self._lib.tpe_get_split_info(self._h, C.byref(info)))
         return int(info.n_below_all), int(info.n_below_obs), int(info.n_above_obs)
 
+    # -- analysis ----------------------------------------------------------------------------------
+    def hypervolume_history(self, values, feasible, ref) -> np.ndarray:
+        """Hypervolume after each trial of ``values`` [n, M] (sign-normalised, trial order) against the
+        sign-normalised reference point ``ref`` [M]; ``feasible`` [n] bools or None (all feasible).  Leaves the
+        history and the suggestion state of this engine unchanged (tpe_hypervolume_history)."""
+        v = _f64(values)
+        r = _f64(ref).reshape(-1)
+        if v.ndim != 2 or v.shape[1] != r.size:
+            raise ValueError(f"values must be [n, {r.size}], got shape {v.shape}")
+        f = None
+        if feasible is not None:
+            f = np.ascontiguousarray(feasible, dtype=np.uint8).reshape(-1)
+            if f.size != v.shape[0]:
+                raise ValueError(f"feasible has {f.size} entries for {v.shape[0]} trials")
+        out = np.empty(v.shape[0], dtype=np.float64)
+        self._check(self._lib.tpe_hypervolume_history(self._h, _ptr(v), _ptr(f), v.shape[0], r.size, _ptr(r),
+                                                      _ptr(out)))
+        return out
+
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:
         below = np.empty(self._info[1], dtype=np.int64)
