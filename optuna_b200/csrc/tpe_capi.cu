@@ -28,8 +28,6 @@
 // environment variables.  Some of them switch parts of the
 // log-sum-exp off (wrong results by design).  The product library contains none of them.
 #ifdef TPE_LAB
-#include "tpe_mma2.cuh"
-#include "tpe_mma3.cuh"
 #include "tpe_screen.cuh"
 #endif
 
@@ -314,7 +312,7 @@ struct MmaInst {
   static void launch(dim3 grid, size_t sm, cudaStream_t st, const void* tab, const double* cst, int64_t Kf,
                      const double2* colprm, const double* xT, int64_t ct_stride, int64_t kps, double skip,
                      double2* part, unsigned long long* gmax) {
-    // near tier: within ln K + 17.5 of the reference max (see LseTier); TPE_TNEAR_DELTA shrinks it for
+    // near tier: within ln K + 17.5 of the reference max (see LseRef); TPE_TNEAR_DELTA shrinks it for
     // timing experiments only (the accuracy bound no longer holds)
 #ifdef TPE_LAB
     static const double delta = [] { const char* v = getenv("TPE_TNEAR_DELTA"); return v ? atof(v) : 0.0; }();
@@ -332,57 +330,6 @@ struct MmaInst {
   static FastCfg cfg() { return FastCfg{PB, (NT / 32) * 8 * M, NT, TK, ST, MINB, smem, &launch, &prepare}; }
 };
 #ifdef TPE_LAB
-// round-2 kernel (tpe_mma2.cuh): OPT bit 0 = seeded base, bit 1 = pipelined classification
-template <int PB, int M, int KG, int NT, int TK, int ST, int MINB, int OPT>
-struct MmaInst2 {
-  static constexpr size_t smem = (size_t)ST * TK * PB * 8 + (size_t)ST * TK * 8 + (size_t)ST * 16;
-  static void launch(dim3 grid, size_t sm, cudaStream_t st, const void* tab, const double* cst, int64_t Kf,
-                     const double2* colprm, const double* xT, int64_t ct_stride, int64_t kps, double skip,
-                     double2* part, unsigned long long* gmax) {
-    // OPT bit 2 (budgeted log-sum-exp): the last argument is the fp32-tier budget of one lane, 2e-7 / (4 * k-splits)
-    const double last = (OPT & 4) ? 2e-7 / (4.0 * grid.y) : skip - 12.5;
-    k_logpdf_mma2<PB, M, KG, NT, TK, ST, MINB, OPT><<<grid, NT, sm, st>>>(static_cast<const double*>(tab), cst, Kf, colprm,
-                                                                         xT, ct_stride, kps, skip, part, gmax, last);
-  }
-  static cudaError_t prepare() {
-    return cudaFuncSetAttribute(k_logpdf_mma2<PB, M, KG, NT, TK, ST, MINB, OPT>,
-                                cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-  }
-  static FastCfg cfg() { return FastCfg{PB, (NT / 32) * 8 * M, NT, TK, ST, MINB, smem, &launch, &prepare}; }
-};
-// warp-compacted exact tier (tpe_mma3.cuh)
-template <int PB, int KG, int NT, int TK, int ST, int MINB>
-struct MmaInst3 {
-  static constexpr size_t smem = (size_t)ST * TK * PB * 8 + (size_t)ST * TK * 8 + (size_t)ST * 16 + (size_t)(NT / 32) * kQWarpBytes;
-  static void launch(dim3 grid, size_t sm, cudaStream_t st, const void* tab, const double* cst, int64_t Kf,
-                     const double2* colprm, const double* xT, int64_t ct_stride, int64_t kps, double skip,
-                     double2* part, unsigned long long* gmax) {
-    k_logpdf_mma3<PB, KG, NT, TK, ST, MINB><<<grid, NT, sm, st>>>(static_cast<const double*>(tab), cst, Kf, colprm, xT,
-                                                                 ct_stride, kps, skip, part, gmax, skip - 12.5);
-  }
-  static cudaError_t prepare() {
-    return cudaFuncSetAttribute(k_logpdf_mma3<PB, KG, NT, TK, ST, MINB>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)smem);
-  }
-  static FastCfg cfg() { return FastCfg{PB, (NT / 32) * 8, NT, TK, ST, MINB, smem, &launch, &prepare}; }
-};
-const FastCfg kMma32V3[] = {
-    MmaInst3<32, 2, 512, 128, 3, 2>::cfg(),  // i
-    MmaInst3<32, 4, 256, 128, 3, 2>::cfg(),  // j: 4 kernel groups in flight, 16 warps / SM
-    MmaInst3<32, 2, 256, 128, 3, 3>::cfg(),  // k: 3 CTAs x 8 warps
-};
-const FastCfg kMma32V2[] = {
-    MmaInst2<32, 1, 2, 512, 128, 3, 2, 1>::cfg(),  // 8: seed
-    MmaInst2<32, 1, 2, 512, 128, 3, 2, 3>::cfg(),  // 9: seed + pipe
-    MmaInst2<32, 1, 2, 512, 128, 3, 2, 2>::cfg(),  // a: pipe
-    MmaInst2<32, 1, 4, 256, 128, 3, 2, 3>::cfg(),  // b: seed + pipe, 4 kernel groups in flight, 16 warps / SM
-    MmaInst2<32, 1, 2, 256, 128, 3, 3, 3>::cfg(),  // c: seed + pipe, 3 CTAs x 8 warps
-    MmaInst2<32, 1, 2, 512, 128, 3, 2, 4>::cfg(),  // d: budgeted log-sum-exp
-    MmaInst2<32, 1, 2, 512, 128, 3, 2, 5>::cfg(),  // e: budgeted + seed
-    MmaInst2<32, 1, 4, 256, 128, 3, 2, 5>::cfg(),  // f: budgeted + seed, KG = 4, 16 warps / SM
-    MmaInst2<32, 1, 2, 512, 128, 3, 2, 8>::cfg(),  // g: near terms parked in a lane-private local-memory buffer
-    MmaInst2<32, 1, 2, 512, 128, 3, 2, 9>::cfg(),  // h: g + seed
-};
 #endif  // TPE_LAB
 // Tilings measured on an H100 SXM (400 W power limit, 1980 MHz max SM clock), CUDA events around the g(x)
 // launch, 100k kernels (tools/tune_mma.py).  M = 2 issues mma.m16n8k8 (twice the m8n8k4 rate on H100), M = 1
@@ -392,8 +339,8 @@ const FastCfg kMma32V2[] = {
 //   P = 16: 1.18 ms (m8n8k4: 1.27)   P = 32: 1.14 ms (m8n8k4: 1.41)   P = 64: 1.77 ms (m8n8k4: 2.15)
 //   P = 8: m8n8k4 stays faster: 1.151-1.154 ms against 1.190 ms for the best m16n8k8 tiling in three alternated
 //   pairs of runs (the means of one tiling spread by 0.003 ms, the gap is 0.037 ms).
-// Small path (one ask of 24 candidates): m8n8k4 stays (the best m16n8k8 tiling is no faster at P = 64 and
-// 14-30 % slower at the other widths).
+// Small path (one ask of 24 candidates): m8n8k4 stays at P <= 32 (14-30 % faster there).  At P = 64 m16n8k8 wins
+// since the steps are software-pipelined: 0.061 against 0.065 ms (H100 SXM, 400 W).
 //                                   PB M KG  NT   TK ST MINB
 const FastCfg kMmaBig[] = {
     MmaInst<8, 1, 4, 256, 512, 3, 2>::cfg(), MmaInst<16, 2, 2, 256, 256, 3, 2>::cfg(),
@@ -401,7 +348,7 @@ const FastCfg kMmaBig[] = {
 };
 const FastCfg kMmaSmall[] = {
     MmaInst<8, 1, 4, 64, 512, 3, 4>::cfg(), MmaInst<16, 1, 4, 64, 256, 3, 4>::cfg(),
-    MmaInst<32, 1, 4, 64, 128, 3, 4>::cfg(), MmaInst<64, 1, 2, 64, 64, 3, 3>::cfg(),
+    MmaInst<32, 1, 4, 64, 128, 3, 4>::cfg(), MmaInst<64, 2, 2, 64, 64, 3, 3>::cfg(),
 };
 #ifdef TPE_LAB
 const FastCfg kMma32Variants[] = {
@@ -411,8 +358,8 @@ const FastCfg kMma32Variants[] = {
     MmaInst<32, 1, 2, 512, 128, 3, 2, 2>::cfg(), MmaInst<32, 1, 4, 256, 128, 3, 2, 1>::cfg(),
 };
 // Tilings for every width, big and small path, selected by TPE_MMA_LAB=<index> when the width matches
-// (tools/tune_mma.py); DBG = 1 / 2 time the mma + TMA floor and the classification + far tier alone, DBG = 3
-// starts the accumulator at ckk - base (no per-term DADD before the classification).
+// (tools/tune_mma.py); DBG = 1 / 2 time the mma + TMA floor and the classification + far tier alone, DBG = 4 the mma +
+// TMA floor without the per-tile exchange of maxima (sync_global).
 //                                   PB M KG  NT   TK ST MINB DBG
 const FastCfg kMmaLab[] = {
     MmaInst<32, 1, 2, 256, 128, 2, 3, 1>::cfg(),  //  0
@@ -445,7 +392,7 @@ const FastCfg kMmaLab[] = {
     MmaInst<64, 2, 1, 256, 64, 2, 2>::cfg(),      // 27
     MmaInst<64, 2, 1, 64, 64, 3, 3>::cfg(),       // 28  small
     MmaInst<64, 2, 2, 64, 64, 3, 3>::cfg(),       // 29  small
-    MmaInst<32, 2, 1, 256, 128, 2, 2, 3>::cfg(),  // 30  accumulator initialised with ckk - base
+    MmaInst<32, 2, 1, 256, 128, 2, 2, 4>::cfg(),  // 30  as 7, without the per-tile exchange of maxima
 };
 constexpr int kMmaLabN = sizeof(kMmaLab) / sizeof(kMmaLab[0]);
 #endif  // TPE_LAB
@@ -460,10 +407,6 @@ const FastCfg* pick_mma(int pb, int64_t Ct) {
   if (pb == 32 && !small) {
     const char* v = getenv("TPE_MMA_VARIANT");
     if (v && v[0] >= '0' && v[0] <= '7') return &kMma32Variants[v[0] - '0'];
-    if (v && v[0] == '8') return &kMma32V2[0];
-    if (v && v[0] == '9') return &kMma32V2[1];
-    if (v && v[0] >= 'a' && v[0] <= 'h') return &kMma32V2[2 + (v[0] - 'a')];
-    if (v && v[0] >= 'i' && v[0] <= 'k') return &kMma32V3[v[0] - 'i'];
   }
 #endif
   const FastCfg* tabs = small ? kMmaSmall : kMmaBig;

@@ -1463,132 +1463,130 @@ __device__ __forceinline__ float ex2_approx(float x) {
   asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(x));
   return y;
 }
-// Two-tier log-sum-exp for the tensor-core kernel.  Terms are classified against a reference `base`
-// (a lower bound of the candidate's true max: the lane's own max or one published by another lane /
-// CTA):
-//   near  L - base > -tnear           parked and folded exactly in fp64 (as LseAcc)
-//   far   -skip < L - base <= -tnear  exp() evaluated at once with the fp32 SFU path (MUFU.EX2) and summed
-//                                     relative to base: no parking, no fp64 work, branch-free
+// e^x for -700 <= x <= 700 in ~17 instructions: x = (64 n + j) ln2 / 64 + r, |r| <= ln2 / 128;
+// e^x = 2^n * 2^(j/64) * P5(r) with a 64-entry table in shared memory (filled by the CTA: exp2(j / 64), 1 ulp) and a
+// degree-5 Taylor polynomial (truncation 3.5e-17).  The two-term Cody-Waite reduction is exact for |x| < 700
+// (ln2_hi / 64 keeps 21 trailing zero bits).  Relative error <= 3e-16.
+__device__ __forceinline__ double uni_exp(double x, const double* __restrict__ tab64) {
+  const double t = fma(x, 92.332482616893656768, 6755399441055744.0);
+  const int ni = __double2loint(t);
+  const double nf = t - 6755399441055744.0;
+  double r = fma(nf, -1.08304246932675596327e-02, x);
+  r = fma(nf, -2.98158582698529328128e-12, r);
+  double p = 8.33333333333333333333e-03;
+  p = fma(p, r, 4.16666666666666666667e-02);
+  p = fma(p, r, 1.66666666666666666667e-01);
+  p = fma(p, r, 0.5);
+  p = fma(p, r, 1.0);
+  p = fma(p, r, 1.0);
+  const double y = tab64[ni & 63] * p;
+  return __hiloint2double(__double2hiint(y) + ((ni >> 6) << 20), __double2loint(y));
+}
+
+// Two-tier log-sum-exp of the tensor-core kernel, summed against a fixed reference R.  Terms are classified against
+// `base`, a lower bound of the candidate's true max (the largest term this lane has folded, or a larger one published
+// by another lane / CTA):
+//   near  L - base > -tnear           parked, then e^(L - R) in fp64 (uni_exp) by the whole warp at once
+//   far   -skip < L - base <= -tnear  e^(L - R) at once on the fp32 SFU path (MUFU.EX2), summed in fp32:
+//                                     no parking, no fp64 work, branch-free
 //   else  dropped
-// With tnear = ln K + 17.5 and skip = ln K + 30 the result stays inside the fp64-parity budget
-// whatever the data: each far term is <= e^-tnear of the max term, there are <= K of them and each
-// carries <= 7.5e-6 relative error (fp32 rounding of L - base: 1.9e-6 for |L - base| < 64; rounding of
-// the product with log2 e and of that constant: 3.2e-6; ex2.approx: 2.4e-7; fp32 runs of <= 32 terms:
-// 1.9e-6), so the far tier adds <= 7.5e-6 * K * e^-tnear = 1.9e-13 relative to the sum; dropped terms
-// add <= 1e-13.
-// At config 2 ~80 % of the terms inside the skip window are far: the exact folds (a full fp64 exp
-// each, executed by the whole warp) become ~5x rarer.
-struct LseTier {
-  double m, s, base, gm, fsum, b0, b1, b2, b3;
-  float ffar;
+// With tnear = ln K + 17.5 and skip = ln K + 30 the result stays inside the fp64-parity budget whatever the data:
+// each far term is <= e^-tnear of the max term, there are <= K of them and each carries <= 7.5e-6 relative error
+// (fp32 rounding of L - R: 1.9e-6 for |L - R| < 64; rounding of the product with log2 e and of that constant:
+// 3.2e-6; ex2.approx: 2.4e-7; fp32 runs of <= 32 terms: 1.9e-6), so the far tier adds <= 7.5e-6 * K * e^-tnear =
+// 1.9e-13 relative to the sum; dropped terms add <= 1e-13.  The thresholds are compared in fp32 (against
+// fl(base - R) - tnear), which moves them by < 1e-5 nats: a factor e^1e-5 on these bounds.
+// R is the first value base takes and moves (to base, with one rescale of the sum) only when base climbs more than
+// kRefMove above it, so R <= base <= R + kRefMove at all times.  Hence a far term has -skip < L - R <= kRefMove -
+// tnear (|L - R| < 64 for any K <= e^34), a near term e^(L - R) <= e^kRefMove, and the exact terms need no running
+// max: they are independent exponentials, and a rise of base costs no rescale.
+constexpr double kRefMove = 48.0;
+struct LseRef {
+  double R, s, base;     // reference, sum of e^(L - R), classification base
+  double b0, b1, b2, b3; // parked near terms
+  float ffar;            // current fp32 run of far terms, relative to R
+  float thn;             // near threshold on fl(L - R): fl(base - R) - tnear (far: - skip)
   int cnt;
   __device__ __forceinline__ void init() {
-    m = -INFINITY; s = 0.0; base = -INFINITY; gm = -INFINITY; fsum = 0.0;
-    b0 = b1 = b2 = b3 = 0.0; ffar = 0.0f; cnt = 0;
+    R = -INFINITY; s = 0.0; base = -INFINITY; b0 = b1 = b2 = b3 = 0.0;
+    ffar = 0.0f; thn = -INFINITY; cnt = 0;   // cold: every finite term is near
   }
-  // e^x for x <= 0 (the only arguments a running log-sum-exp needs): one range reduction, a
-  // degree-12 Taylor polynomial on |r| <= ln2 / 2 (truncation 2e-16) and an exponent add -- ~20
-  // instructions instead of the ~45 of the general exp().  x < -700 (incl. -inf) returns 0.
-  static __device__ __forceinline__ double exp_neg(double x) {
-    const double xc = fmax(x, -700.0);
-    const double t = fma(xc, 1.4426950408889634074, 6755399441055744.0);
-    const int n = __double2loint(t);
-    const double nf = t - 6755399441055744.0;
-    double r = fma(nf, -6.93147180369123816490e-01, xc);
-    r = fma(nf, -1.90821492927058770002e-10, r);
-    double p = 2.08767569878680989792e-09;           // 1 / 12!
-    p = fma(p, r, 2.50521083854417187751e-08);       // 1 / 11!
-    p = fma(p, r, 2.75573192239858906526e-07);
-    p = fma(p, r, 2.75573192239858906526e-06);
-    p = fma(p, r, 2.48015873015873015873e-05);
-    p = fma(p, r, 1.98412698412698412698e-04);
-    p = fma(p, r, 1.38888888888888888889e-03);
-    p = fma(p, r, 8.33333333333333333333e-03);
-    p = fma(p, r, 4.16666666666666666667e-02);
-    p = fma(p, r, 1.66666666666666666667e-01);
-    p = fma(p, r, 0.5);
-    p = fma(p, r, 1.0);
-    p = fma(p, r, 1.0);
-    const double y = __hiloint2double(__double2hiint(p) + (n << 20), __double2loint(p));
-    return (x < -700.0) ? 0.0 : y;
+  // base := nb (>= base); R follows when nb is more than kRefMove above it (also the cold start, R = -inf: s and the
+  // far run are 0 then).  Executed by the whole warp together.
+  __device__ __forceinline__ void rebase(double nb, float tnear, const double* e64) {
+    if (__any_sync(0xffffffffu, nb > R + kRefMove)) {
+      const bool mv = nb > R + kRefMove;
+      const double f = uni_exp(fmax(R - nb, -700.0), e64);
+      s = mv ? (s + (double)ffar) * f : s;
+      ffar = mv ? 0.0f : ffar;
+      R = mv ? nb : R;
+    }
+    base = nb;
+    const float d = __double2float_rn(base - R);   // R = -inf only while base = -inf: stay cold
+    thn = (R == -INFINITY) ? -INFINITY : d - tnear;
   }
-  // fold the parked terms: new max first, then the rescale factor and the (up to 4) terms are
-  // independent exps.  Then bring the far-tier sum (relative to base) into (m, s) and move base up
-  // to the best max known.  Executed by the whole warp together.
-  __device__ __forceinline__ void flush() {
+  // fold the parked terms (executed by the whole warp together): base first, then up to 4 independent exps
+  __device__ __forceinline__ void flush(float tnear, const double* e64) {
     const bool v0 = cnt > 0, v1 = cnt > 1, v2 = cnt > 2, v3 = cnt > 3;
-    double nm = m;
-    nm = (v0 && b0 > nm) ? b0 : nm;
-    nm = (v1 && b1 > nm) ? b1 : nm;
-    nm = (v2 && b2 > nm) ? b2 : nm;
-    nm = (v3 && b3 > nm) ? b3 : nm;
-    // m = -inf (nothing folded yet): s = 0 and exp_neg(-inf or NaN) is finite, so the product is 0
-    double t = s * exp_neg(m - nm);
-    const double e0 = exp_neg(b0 - nm), e1 = exp_neg(b1 - nm), e2 = exp_neg(b2 - nm), e3 = exp_neg(b3 - nm);
-    t += (v0 ? e0 : 0.0) + (v1 ? e1 : 0.0);
-    t += (v2 ? e2 : 0.0) + (v3 ? e3 : 0.0);
-    s = t;
-    m = nm;
+    double nb = base;
+    nb = (v0 && b0 > nb) ? b0 : nb;
+    nb = (v1 && b1 > nb) ? b1 : nb;
+    nb = (v2 && b2 > nb) ? b2 : nb;
+    nb = (v3 && b3 > nb) ? b3 : nb;
+    rebase(nb, tnear, e64);
+    // stale slots may hold anything: selected away, never multiplied
+    const double e0 = uni_exp(fmax(b0 - R, -700.0), e64), e1 = uni_exp(fmax(b1 - R, -700.0), e64);
+    const double e2 = uni_exp(fmax(b2 - R, -700.0), e64), e3 = uni_exp(fmax(b3 - R, -700.0), e64);
+    s += ((v0 ? e0 : 0.0) + (v1 ? e1 : 0.0)) + ((v2 ? e2 : 0.0) + (v3 ? e3 : 0.0));
     cnt = 0;
-    const double fs = fsum + (double)ffar;
-    fsum = 0.0;
-    ffar = 0.0f;
-    const bool own = m >= base;                    // also the cold start (base = -inf)
-    const bool adopt = !own && fs != 0.0;          // only far terms so far: take base as the reference
-    const double ex = exp_neg(-fabs(m - base));    // m or base = -inf: 0
-    const double s_own = (fs != 0.0) ? fma(fs, ex, s) : s;   // base = -inf implies fs = 0
-    const double s_adopt = fma(s, ex, fs);
-    s = own ? s_own : (adopt ? s_adopt : s);
-    m = adopt ? base : m;
-    base = fmax(m, gm);
   }
   __device__ __forceinline__ void roll() {  // bounds the length of the fp32 runs (once per tile)
-    fsum += (double)ffar;
+    s += (double)ffar;
     ffar = 0.0f;
   }
-  __device__ __forceinline__ void sync_global(unsigned long long* slot) {
-    if (m > gm) atomicMax(slot, static_cast<unsigned long long>(order_bits(m)));
+  // Publish base in `slot` (ordered-integer atomicMax) and adopt a larger one published by the k-splits and lanes
+  // that share the candidate.  Any published value is some kernel's L, hence <= the true max.
+  __device__ __forceinline__ void sync_global(unsigned long long* slot, float tnear, const double* e64) {
     const double seen = from_order_bits(*reinterpret_cast<volatile unsigned long long*>(slot));
-    gm = fmax(gm, seen);
-    if (__any_sync(0xffffffffu, gm > base)) flush();
+    if (base > seen) atomicMax(slot, static_cast<unsigned long long>(order_bits(base)));
+    if (__any_sync(0xffffffffu, seen > base)) rebase(fmax(base, seen), tnear, e64);
   }
-  __device__ __forceinline__ void park(double L, bool near) {
+  __device__ __forceinline__ void park(double L, bool near, float tnear, const double* e64) {
     b3 = near ? b2 : b3;
     b2 = near ? b1 : b2;
     b1 = near ? b0 : b1;
     b0 = near ? L : b0;
     cnt += near ? 1 : 0;
-    if (__any_sync(0xffffffffu, cnt == 4)) flush();
+    if (__any_sync(0xffffffffu, cnt == 4)) flush(tnear, e64);
   }
-  // N terms at once: the classification and the far-tier exps of all of them are independent
-  // (pipelined through the fp64 / SFU / fp32 pipes), one vote decides whether any lane has a near
-  // term at all -- rare once base has converged (< 1 % of the terms are near).
-  // SHIFTED (timing experiment): L holds L - sh, with sh = base (or 0 while base = -inf), so the classification
-  // needs no DADD and L is rebuilt only for the parked terms.
-  template <int N, bool EXACT, bool SHIFTED = false>
-  __device__ __forceinline__ void push_batch(const double (&L)[N], float skip, float tnear, double sh = 0.0) {
-    bool near[N];
+  // One term's classification, independent of every other term's (so the kernel interleaves it with the mma chain
+  // of the next step): adds a far term to `add` (the caller folds it into ffar) and says whether the term is near.
+  // gap = skip - tnear.
+  __device__ __forceinline__ bool classify(double L, float gap, float& add) const {
+    const float df = __double2float_rn(L - R);  // cold (R = -inf): +inf -> near; L = -inf or NaN: dropped
+    const bool near = df > thn;
+    const bool far = !near && df > thn - gap;
+    const float e = ex2_approx(df * 1.44269504f);
+    add += far ? e : 0.0f;
+    return near;
+  }
+  // park the near terms of one batch; one vote decides whether any lane has a near term at all.  Terms of the batch
+  // classified far against the old base stay far (exact enough by construction) even if a flush raises base.
+  template <int N>
+  __device__ __forceinline__ void park_batch(const double (&L)[N], const bool (&near)[N], float tnear,
+                                             const double* e64) {
     bool any = false;
-    float add = 0.0f;
-    const bool cold = SHIFTED && base == -INFINITY;
 #pragma unroll
-    for (int i = 0; i < N; ++i) {
-      const float df = SHIFTED ? (cold ? INFINITY : __double2float_rn(L[i]))
-                               : __double2float_rn(L[i] - base);  // base = -inf -> +inf -> near
-      near[i] = df > -tnear;
-      const bool far = !near[i] && df > -skip;
-      const float e = ex2_approx(df * 1.44269504f);
-      add += far ? e : 0.0f;
-      any = any || near[i];
-    }
-    ffar += add;
-    if (EXACT && __any_sync(0xffffffffu, any)) {
-      // note: terms of this batch that were classified far against the old base stay far (exact
-      // enough by construction) even if a flush below raises base
+    for (int i = 0; i < N; ++i) any = any || near[i];
+    if (__any_sync(0xffffffffu, any)) {
 #pragma unroll
       for (int i = 0; i < N; ++i)
-        if (__any_sync(0xffffffffu, near[i])) park(SHIFTED ? L[i] + sh : L[i], near[i]);
+        if (__any_sync(0xffffffffu, near[i])) park(L[i], near[i], tnear, e64);
     }
+  }
+  // the lane's (max, sum) pair for lse_merge, relative to base (s e^(R - base); R = base = -inf: (-inf, 0))
+  __device__ __forceinline__ double2 result(const double* e64) const {
+    return make_double2(base, s * uni_exp(fmax(R - base, -700.0), e64));
   }
 };
 
@@ -1630,9 +1628,10 @@ __device__ __forceinline__ void dmma_16x8x8(double& d0, double& d1, double& d2, 
                : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3)
                : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
 }
-// KG kernel groups (8 kernels each) are in flight per warp: KG * M independent m8n8k4 chains (M = 1), or
-// KG * M / 2 m16n8k8 chains (M even, two candidate groups per instruction), which is what keeps the DMMA
-// pipe fed (one chain of dependent DMMAs alone cannot hide the DMMA latency).
+// KG kernel groups (8 kernels each) per step of a warp: KG * M independent m8n8k4 chains (M = 1), or KG * M / 2
+// m16n8k8 chains (M even, two candidate groups per instruction).  The steps are software-pipelined: a warp issues
+// the chains of step s + 1 before it classifies the sums of step s, so the DMMA latency of one step hides behind
+// the log-sum-exp of the previous one (two accumulator sets live at once).
 template <int PB, int M, int KG, int NT, int TK, int ST, int MINB, int DBG = 0>
 __global__ void __launch_bounds__(NT, MINB)
 k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, int64_t Kfp,
@@ -1643,6 +1642,7 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
   constexpr int NI = PB / 4;        // k-steps of the mma chain
   constexpr int CW = 8 * M;         // candidates per warp
   extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ double s_e64[64];                                                     // uni_exp table
   double* tiles = reinterpret_cast<double*>(smem_raw);                             // ST * TK * PB
   double* csts = tiles + (size_t)ST * TK * PB;                                     // ST * TK
   uint64_t* full = reinterpret_cast<uint64_t*>(csts + (size_t)ST * TK);            // ST
@@ -1653,8 +1653,10 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
   const int64_t k0 = blockIdx.y * kps;
   const int64_t k1 = (k0 + kps < Kfp) ? k0 + kps : Kfp;   // Kfp, kps: multiples of 8 * KG
   const int ntiles = (k1 > k0) ? (int)((k1 - k0 + TK - 1) / TK) : 0;
+  const int nsteps = (k1 > k0) ? (int)((k1 - k0) / (8 * KG)) : 0;
   const int64_t wbase = (int64_t)blockIdx.x * ((NT / 32) * CW) + (int64_t)(tid >> 5) * CW;
 
+  if (tid < 64) s_e64[tid] = exp2((double)tid * 0.015625);
   if (tid == 0) {
     for (int s = 0; s < ST; ++s) {
       mbar_init(&full[s], 1);
@@ -1677,6 +1679,18 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
   if (tid == 0) {
     for (int t = 0; t < ST - 1 && t < ntiles; ++t) issue(t);
   }
+  // make tile t readable; the stage being refilled held tile t - 1: first wait until every warp has released it
+  auto enter = [&](int t) {
+    if (tid == 0 && t + ST - 1 < ntiles) {
+      if (t > 0) mbar_wait(&empty[(t - 1) % ST], (uint32_t)(((t - 1) / ST) & 1));
+      issue(t + ST - 1);
+    }
+    mbar_wait(&full[t % ST], (uint32_t)((t / ST) & 1));
+  };
+  auto groups_in = [&](int t) {  // kernel groups of tile t
+    const int64_t ks = k0 + (int64_t)t * TK;
+    return (int)((k1 - ks < TK) ? (k1 - ks) : TK) / 8;
+  };
 
   // A fragments: a[m][i] = A[row g][col q] of k-step i = scaled coordinate 4 i + q of candidate 8 m + g
   double a[M][NI];
@@ -1701,102 +1715,148 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
     ha[m] += __shfl_xor_sync(0xffffffffu, ha[m], 2);
     ha[m] *= -0.5;
   }
-  LseTier acc[M];
+
+  // The mma chains of kernel groups kg .. kg + KG - 1 of tile t: d[u][m] = C[candidate 8 m + g][kernels 2q, 2q + 1].
+  // work(i) runs after the DMMAs of dependent level i (NL levels): the warp issues in order, so independent work placed
+  // there fills the DMMA latency instead of a stall before the next level.
+  constexpr int NL = (M % 2 == 0) ? NI / 2 : NI;
+  auto chain = [&](int t, int kg, double (&d)[KG][M][2], auto&& work) {
+    const double* tile = tiles + (size_t)(t % ST) * TK * PB;
+    const double* ctile = csts + (size_t)(t % ST) * TK;
+    const double2* fb = reinterpret_cast<const double2*>(tile + (size_t)kg * 8 * PB) + lane;
+#pragma unroll
+    for (int u = 0; u < KG; ++u) {
+      const double2 cc = reinterpret_cast<const double2*>(ctile + (kg + u) * 8)[q];
+#pragma unroll
+      for (int m = 0; m < M; ++m) {
+        d[u][m][0] = cc.x;
+        d[u][m][1] = cc.y;
+      }
+    }
+    double2 v[2][KG];
+#pragma unroll
+    for (int u = 0; u < KG; ++u) v[0][u] = fb[u * (4 * PB)];   // one kernel group = 8 * PB doubles
+#pragma unroll
+    for (int i2 = 0; i2 < NI / 2; ++i2) {
+      if (i2 + 1 < NI / 2) {
+#pragma unroll
+        for (int u = 0; u < KG; ++u) v[(i2 + 1) & 1][u] = fb[u * (4 * PB) + (i2 + 1) * 32];
+      }
+      if constexpr (M % 2 == 0) {
+#pragma unroll
+        for (int u = 0; u < KG; ++u)
+#pragma unroll
+          for (int m = 0; m < M; m += 2)
+            dmma_16x8x8(d[u][m][0], d[u][m][1], d[u][m + 1][0], d[u][m + 1][1], a[m][2 * i2], a[m + 1][2 * i2],
+                        a[m][2 * i2 + 1], a[m + 1][2 * i2 + 1], v[i2 & 1][u].x, v[i2 & 1][u].y);
+        work(i2);
+      } else {
+#pragma unroll
+        for (int u = 0; u < KG; ++u) dmma_8x8x4(d[u][0][0], d[u][0][1], a[0][2 * i2], v[i2 & 1][u].x);
+        work(2 * i2);
+#pragma unroll
+        for (int u = 0; u < KG; ++u) dmma_8x8x4(d[u][0][0], d[u][0][1], a[0][2 * i2 + 1], v[i2 & 1][u].y);
+        work(2 * i2 + 1);
+      }
+    }
+  };
+
+  LseRef acc[M];
 #pragma unroll
   for (int m = 0; m < M; ++m) acc[m].init();
-  const float lim_skip = (float)lse_skip, lim_near = (float)lse_near;
+  const float lim_near = (float)lse_near, lim_gap = (float)(lse_skip - lse_near);
 
-  for (int t = 0; t < ntiles; ++t) {
-    const int st = t % ST;
-    if (tid == 0 && t + ST - 1 < ntiles) {
-      // the stage being refilled held tile t - 1: wait until every warp has released it
-      if (t > 0) mbar_wait(&empty[(t - 1) % ST], (uint32_t)(((t - 1) / ST) & 1));
-      issue(t + ST - 1);
-    }
-    mbar_wait(&full[st], (uint32_t)((t / ST) & 1));
-    const int64_t ks = k0 + (int64_t)t * TK;
-    const int tk = (int)((k1 - ks < TK) ? (k1 - ks) : TK);
-    const double* tile = tiles + (size_t)st * TK * PB;
-    const double* ctile = csts + (size_t)st * TK;
-    for (int kg = 0; kg < tk / 8; kg += KG) {
-      if (kg == 0 || t == 0) {  // every tile, and every iteration of the CTA's first tile (cold start)
+  constexpr int NV = 2 * KG * M;   // sums per lane and step: value j = (m, u, h) = (j / 2KG, j % 2KG / 2, j % 2)
+  double cur[KG][M][2], nxt[KG][M][2];
+  int tc = 0, kc = 0;            // tile and first kernel group of the step in `cur`
+  int ngc = 0;                   // kernel groups of tile tc
+  auto none = [](int) {};
+  if (nsteps > 0) {
+    enter(0);
+    ngc = groups_in(0);
+    chain(0, 0, cur, none);
+  }
+  for (int s = 0; s < nsteps; ++s) {
+    if constexpr (DBG != 4) {
+      if (kc == 0 || tc == 0) {  // every tile, and every step of the CTA's first tile (cold start)
 #pragma unroll
         for (int m = 0; m < M; ++m) {
           acc[m].roll();
-          acc[m].sync_global(gmax + wbase + 8 * m + g);
+          acc[m].sync_global(gmax + wbase + 8 * m + g, lim_near, s_e64);
         }
-      } else if ((kg & 15) == 0) {  // long tiles (small PB): keep the fp32 runs at <= 32 terms
+      } else if ((kc & 15) == 0) {  // long tiles (small PB): keep the fp32 runs at <= 32 terms
 #pragma unroll
         for (int m = 0; m < M; ++m) acc[m].roll();
       }
-      const double2* fb = reinterpret_cast<const double2*>(tile + (size_t)kg * 8 * PB) + lane;
-      double d0[KG][M], d1[KG][M];
-      double sh[M];  // DBG = 3 (timing experiment): the accumulator starts at ckk - base
+    }
+    // classification of value j (far terms summed at once, near ones flagged); DBG = 1 / 4: plain sums
+    bool nr[M][2 * KG];
+    float add[M];
 #pragma unroll
-      for (int m = 0; m < M; ++m) sh[m] = (DBG == 3 && acc[m].base != -INFINITY) ? acc[m].base : 0.0;
+    for (int m = 0; m < M; ++m) add[m] = 0.0f;
+    auto cls = [&](int j) {
+      const int m = j / (2 * KG), u = (j % (2 * KG)) / 2, h = j & 1;
+      if constexpr (DBG == 1 || DBG == 4) acc[m].s += cur[u][m][h];
+      else nr[m][j % (2 * KG)] = acc[m].classify(cur[u][m][h], lim_gap, add[m]);
+    };
+    // level i of the next chain is followed by the values j with j * NL / NV == i
+    auto work = [&](int i) {
 #pragma unroll
-      for (int u = 0; u < KG; ++u) {
-        const double2 cc = reinterpret_cast<const double2*>(ctile + (kg + u) * 8)[q];
-#pragma unroll
-        for (int m = 0; m < M; ++m) {
-          d0[u][m] = cc.x;
-          d1[u][m] = cc.y;
-          if constexpr (DBG == 3) {
-            d0[u][m] -= sh[m];
-            d1[u][m] -= sh[m];
-          }
-        }
+      for (int j = 0; j < NV; ++j)
+        if (j * NL / NV == i) cls(j);
+    };
+
+    // position of step s + 1; at the end of a tile release its stage (its last chain has read the table)
+    int tn = tc, kn = kc + KG, ngn = ngc;
+    if (kn == ngc) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&empty[tc % ST]);
+      tn = tc + 1;
+      kn = 0;
+      if (tn < ntiles) {
+        enter(tn);
+        ngn = groups_in(tn);
       }
-      double2 v[2][KG];
+    }
+    if (s + 1 < nsteps) {
+      chain(tn, kn, nxt, work);
+    } else {
 #pragma unroll
-      for (int u = 0; u < KG; ++u) v[0][u] = fb[u * (4 * PB)];   // one kernel group = 8 * PB doubles
-#pragma unroll
-      for (int i2 = 0; i2 < NI / 2; ++i2) {
-        if (i2 + 1 < NI / 2) {
-#pragma unroll
-          for (int u = 0; u < KG; ++u) v[(i2 + 1) & 1][u] = fb[u * (4 * PB) + (i2 + 1) * 32];
-        }
-        if constexpr (M % 2 == 0) {
-#pragma unroll
-          for (int u = 0; u < KG; ++u)
-#pragma unroll
-            for (int m = 0; m < M; m += 2)
-              dmma_16x8x8(d0[u][m], d1[u][m], d0[u][m + 1], d1[u][m + 1], a[m][2 * i2], a[m + 1][2 * i2],
-                          a[m][2 * i2 + 1], a[m + 1][2 * i2 + 1], v[i2 & 1][u].x, v[i2 & 1][u].y);
-        } else {
-#pragma unroll
-          for (int u = 0; u < KG; ++u) dmma_8x8x4(d0[u][0], d1[u][0], a[0][2 * i2], v[i2 & 1][u].x);
-#pragma unroll
-          for (int u = 0; u < KG; ++u) dmma_8x8x4(d0[u][0], d1[u][0], a[0][2 * i2 + 1], v[i2 & 1][u].y);
-        }
-      }
+      for (int j = 0; j < NV; ++j) cls(j);
+    }
+
+    if constexpr (DBG != 1 && DBG != 4) {
 #pragma unroll
       for (int m = 0; m < M; ++m) {
-        double vals[2 * KG];
+        acc[m].ffar += add[m];
+        if constexpr (DBG == 0) {
+          double vals[2 * KG];
 #pragma unroll
-        for (int u = 0; u < KG; ++u) {
-          vals[2 * u] = d0[u][m];
-          vals[2 * u + 1] = d1[u][m];
-        }
-        if constexpr (DBG == 1) {  // timing experiment: no log-sum-exp work at all
-#pragma unroll
-          for (int u = 0; u < 2 * KG; ++u) acc[m].fsum += vals[u];
-        } else if constexpr (DBG == 2) {  // timing experiment: classification + far tier only
-          acc[m].template push_batch<2 * KG, false>(vals, lim_skip, lim_near);
-        } else if constexpr (DBG == 3) {
-          acc[m].template push_batch<2 * KG, true, true>(vals, lim_skip, lim_near, sh[m]);
-        } else {
-          acc[m].template push_batch<2 * KG, true>(vals, lim_skip, lim_near);
+          for (int u = 0; u < KG; ++u) {
+            vals[2 * u] = cur[u][m][0];
+            vals[2 * u + 1] = cur[u][m][1];
+          }
+          acc[m].template park_batch<2 * KG>(vals, nr[m], lim_near, s_e64);
         }
       }
     }
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[st]);  // this warp is done with stage `st`
+#pragma unroll
+    for (int u = 0; u < KG; ++u)
+#pragma unroll
+      for (int m = 0; m < M; ++m) {
+        cur[u][m][0] = nxt[u][m][0];
+        cur[u][m][1] = nxt[u][m][1];
+      }
+    tc = tn;
+    kc = kn;
+    ngc = ngn;
   }
 #pragma unroll
   for (int m = 0; m < M; ++m) {
-    acc[m].flush();
-    double mm = acc[m].m, ss = acc[m].s;
+    acc[m].flush(lim_near, s_e64);
+    acc[m].roll();
+    const double2 r = acc[m].result(s_e64);
+    double mm = r.x, ss = r.y;
 #pragma unroll
     for (int o = 1; o <= 2; o <<= 1) {
       const double m2 = __shfl_xor_sync(0xffffffffu, mm, o), s2 = __shfl_xor_sync(0xffffffffu, ss, o);

@@ -14,33 +14,13 @@
 //   * every warp walks ALL tiles itself (no k-split: the running max of a candidate is found in the tile under it,
 //     first), so far tiles are dismissed against the true scale of the sum, not against a slice-local max.
 // The log-sum-exp is the two-tier one of the multivariate kernels: terms within ln K + 17.5 of the running max in
-// fp64 (LseTier::exp_neg), terms down to ln K + 30 below it through MUFU.EX2 in fp32, the rest dropped; same bounds.
+// fp64 (uni_exp), terms down to ln K + 30 below it through MUFU.EX2 in fp32, the rest dropped; same bounds.
 #pragma once
 #include "tpe_kernels.cuh"
 
 namespace tpe {
 
 constexpr int kUniTile = 128;
-
-// e^x for -700 <= x <= 700 in ~17 instructions: x = (64 n + j) ln2 / 64 + r, |r| <= ln2 / 128;
-// e^x = 2^n * 2^(j/64) * P5(r) with a 64-entry table in shared memory (filled by the CTA: exp2(j / 64), 1 ulp) and a
-// degree-5 Taylor polynomial (truncation 3.5e-17).  The two-term Cody-Waite reduction is exact for |x| < 700
-// (ln2_hi / 64 keeps 21 trailing zero bits).  Relative error <= 3e-16.
-__device__ __forceinline__ double uni_exp(double x, const double* __restrict__ tab64) {
-  const double t = fma(x, 92.332482616893656768, 6755399441055744.0);
-  const int ni = __double2loint(t);
-  const double nf = t - 6755399441055744.0;
-  double r = fma(nf, -1.08304246932675596327e-02, x);
-  r = fma(nf, -2.98158582698529328128e-12, r);
-  double p = 8.33333333333333333333e-03;
-  p = fma(p, r, 4.16666666666666666667e-02);
-  p = fma(p, r, 1.66666666666666666667e-01);
-  p = fma(p, r, 0.5);
-  p = fma(p, r, 1.0);
-  p = fma(p, r, 1.0);
-  const double y = tab64[ni & 63] * p;
-  return __hiloint2double(__double2hiint(y) + ((ni >> 6) << 20), __double2loint(y));
-}
 
 
 struct UniTileMeta {

@@ -2,7 +2,7 @@
 # A/B of the g(x) grid kernel variants at config 2: stage timings (CUDA events) + parity of the log-densities
 # against the default variant (max |diff| of log g over the 4096 candidates of the same ask).
 export TPE_LAB=1   # the variants live in the lab build (libtpe_b200_lab.so)
-for v in ${VARIANTS:-default 8 d e f}; do
+for v in ${VARIANTS:-default 0 1 2 3}; do
   if [ "$v" = default ]; then unset TPE_MMA_VARIANT; else export TPE_MMA_VARIANT=$v; fi
   echo "== variant $v"
   python - <<'PY'
