@@ -36,7 +36,8 @@ extern "C" {
 /* 5: + tpe_suggest_univariate_batch_async / tpe_collect_univariate */
 /* 6: + tpe_set_kernel_shard / tpe_sample_and_partial / tpe_finish_from_partials */
 /* 7: + tpe_hypervolume_history */
-#define TPE_ABI_VERSION 7
+/* 8: + tpe_pareto_front */
+#define TPE_ABI_VERSION 8
 
 enum {
   TPE_OK = 0,
@@ -264,6 +265,13 @@ int tpe_get_mo_weights(tpe_ctx* ctx, double* weights);
  * TPE_E_INVALID.  Uses its own device memory and leaves the context's history and suggestion state alone. */
 int tpe_hypervolume_history(tpe_ctx* ctx, const double* values, const uint8_t* feasible, int64_t n,
                             int32_t n_objectives, const double* ref, double* out);
+/* Pareto front of a set of objective vectors (replaces _is_pareto_front, optuna/study/_multi_objective.py:171-184,
+ * behind Study.best_trials and plot_pareto_front).  values [n, n_objectives]: the candidate rows, multiplied by +1
+ * (minimise) or -1 (maximise).  on_front [n]: 1 iff no row is <= the row in every objective and < in one; identical
+ * rows never dominate each other, so every copy of a front vector is on the front.  IEEE comparisons (-0.0 == 0.0,
+ * +-inf are ordinary values).  1 <= n_objectives <= 16; NaN in values is TPE_E_INVALID.  Uses its own device memory
+ * and leaves the context's history and suggestion state alone. */
+int tpe_pareto_front(tpe_ctx* ctx, const double* values, int64_t n, int32_t n_objectives, uint8_t* on_front);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

@@ -6,14 +6,16 @@ sm_90a CUDA through a C ABI (include/optuna_b200_tpe.h) bound with ctypes.
 """
 from .engine import ParamSpec, TPEEngine  # noqa: F401
 
-__all__ = ["ParamSpec", "TPEEngine", "B200TPESampler", "hypervolume_history", "plot_hypervolume_history"]
+__all__ = ["ParamSpec", "TPEEngine", "B200TPESampler", "hypervolume_history", "plot_hypervolume_history",
+           "best_trials", "pareto_front_info", "plot_pareto_front"]
 
 
 def __getattr__(name):
     if name == "B200TPESampler":
         from .sampler import B200TPESampler
         return B200TPESampler
-    if name in ("hypervolume_history", "plot_hypervolume_history"):
+    if name in ("hypervolume_history", "plot_hypervolume_history", "best_trials", "pareto_front_info",
+                "plot_pareto_front"):
         from . import analysis
         return getattr(analysis, name)
     raise AttributeError(name)

@@ -20,6 +20,7 @@
 #include "tpe_kernels.cuh"
 #include "tpe_motpe_kernels.cuh"
 #include "tpe_hvhist.cuh"
+#include "tpe_pareto.cuh"
 #include "tpe_uni.cuh"
 #include "tpe_mixed.cuh"
 #include "tpe_tcscreen.cuh"
@@ -1836,6 +1837,75 @@ int hv_history_run(tpe_ctx* ctx, const double* values, const uint8_t* feasible, 
   return TPE_OK;
 }
 
+// ---- Pareto front (tpe_pareto.cuh) ---------------------------------------------------------------
+// Device memory of one tpe_pareto_front call, released when it returns: nothing a suggestion reads is touched.
+struct PfScratch {
+  DevBuf v, s, s0, fv, key, idx, work, dom, nf, flags;
+  ~PfScratch() {
+    for (DevBuf* b : {&v, &s, &s0, &fv, &key, &idx, &work, &dom, &nf, &flags}) b->release();
+  }
+};
+
+int pareto_front_run(tpe_ctx* ctx, const double* values, int n, int M, uint8_t* on_front) {
+  cudaStream_t st = ctx->stream;
+  PfScratch b;
+  const size_t vb = (size_t)n * M * 8;
+  for (DevBuf* x : {&b.v, &b.s, &b.fv}) CU(x->ensure(vb));
+  CU(b.s0.ensure((size_t)n * 8));
+  CU(b.key.ensure((size_t)n * 16));
+  CU(b.idx.ensure((size_t)n * 12));
+  CU(b.work.ensure(sizeof(SortWork)));
+  for (DevBuf* x : {&b.dom, &b.flags}) CU(x->ensure((size_t)n));
+  CU(b.nf.ensure(4));
+  CU(cudaMemcpyAsync(b.v.p, values, vb, cudaMemcpyHostToDevice, st));
+  for (DevBuf* x : {&b.dom, &b.flags}) CU(cudaMemsetAsync(x->p, 0, (size_t)n, st));
+  CU(cudaMemsetAsync(b.nf.p, 0, 4, st));
+  // 1. stable order by coordinate 0
+  const double* d_v = b.v.as<double>();
+  int32_t pc = M;
+  int j_col = 0, n_i = n;
+  uint64_t* ka = b.key.as<uint64_t>();
+  uint64_t* kb = ka + n;
+  int32_t* order = b.idx.as<int32_t>();
+  int32_t* ia = order + n;
+  int32_t* ib = ia + n;
+  SortWork* wk = b.work.as<SortWork>();
+  const int* run_flag = nullptr;
+  void* args[] = {&d_v, &pc, &j_col, &n_i, &ka, &kb, &ia, &ib, &wk, &order, &run_flag};
+  int G = std::max(1, std::min(std::min(ctx->sm_count, 160), (n + 1023) / 1024));
+  if (ctx->sort_cta_cap > 0) G = std::min(G, ctx->sort_cta_cap);
+  CU(cudaLaunchCooperativeKernel((const void*)k_radix_sort_coop, dim3(G), dim3(512), args, 0, st));
+  const int64_t nm = (int64_t)n * M;
+  k_pf_gather<<<(unsigned)((nm + 255) / 256), 256, 0, st>>>(d_v, order, n, M, b.s.as<double>(), b.s0.as<double>());
+  CU(cudaGetLastError());
+  // 2. chunks [cuts[c], cuts[c + 1]) of about kPfChunk sorted rows; a tie run of coordinate 0 (==, so -0.0 ties
+  //    with +0.0) is never split
+  std::vector<double> s0((size_t)n);
+  CU(cudaMemcpyAsync(s0.data(), b.s0.p, (size_t)n * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  std::vector<int> cuts{0};
+  while (cuts.back() < n) {
+    int c = std::min(n, cuts.back() + kPfChunk);
+    while (c < n && s0[c] == s0[c - 1]) ++c;
+    cuts.push_back(c);
+  }
+  // 3. filter and append, chunk by chunk; no host round trip (the front size stays on the device)
+  for (size_t c = 0; c + 1 < cuts.size(); ++c) {
+    const int c0 = cuts[c], c1 = cuts[c + 1];
+    const int n_fslices = (c0 + kPfSlice - 1) / kPfSlice;   // the front holds at most c0 rows
+    const int n_slices = n_fslices + (c1 - c0 + kPfSlice - 1) / kPfSlice;
+    const dim3 grid((unsigned)((c1 - c0 + kPfThreads - 1) / kPfThreads), (unsigned)std::min(n_slices, 65535));
+    k_pf_filter<<<grid, kPfThreads, pf_filter_smem(M), st>>>(b.s.as<double>(), c0, c1, M, b.fv.as<double>(),
+                                                             b.nf.as<int>(), n_fslices, b.dom.as<uint8_t>());
+    k_pf_append<<<1, 1024, 0, st>>>(b.s.as<double>(), order, c0, c1, M, b.dom.as<uint8_t>(), b.fv.as<double>(),
+                                    b.nf.as<int>(), b.flags.as<uint8_t>());
+    CU(cudaGetLastError());
+  }
+  CU(cudaMemcpyAsync(on_front, b.flags.p, (size_t)n, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
 
 // =================================================================================================
 extern "C" {
@@ -2098,6 +2168,20 @@ int tpe_hypervolume_history(tpe_ctx* ctx, const double* values, const uint8_t* f
   if (n == 0) return TPE_OK;
   if (set_device(ctx, false)) return TPE_E_CUDA;
   return hv_history_run(ctx, values, feasible, (int)n, M, ref, out);
+}
+
+int tpe_pareto_front(tpe_ctx* ctx, const double* values, int64_t n, int32_t n_objectives, uint8_t* on_front) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  const int M = n_objectives;
+  if (M < 1 || M > kMoMaxM) return fail(ctx, TPE_E_INVALID, "n_objectives must be in [1, %d]", kMoMaxM);
+  if (n < 0 || n >= (1ll << 31) - 4096) return fail(ctx, TPE_E_INVALID, "bad number of rows %lld", (long long)n);
+  if (n > 0 && (!values || !on_front)) return fail(ctx, TPE_E_INVALID, "bad Pareto front arguments");
+  for (int64_t q = 0; q < n * M; ++q)
+    if (std::isnan(values[q])) return fail(ctx, TPE_E_INVALID, "objective values hold NaN (row %lld)", (long long)(q / M));
+  if (n == 0) return TPE_OK;
+  if (set_device(ctx, false)) return TPE_E_CUDA;
+  return pareto_front_run(ctx, values, (int)n, M, on_front);
 }
 
 int64_t tpe_history_size(tpe_ctx* ctx) { return ctx ? ctx->N : -1; }

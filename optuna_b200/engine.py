@@ -380,6 +380,17 @@ class TPEEngine:
                                                       _ptr(out)))
         return out
 
+    def pareto_front(self, values) -> np.ndarray:
+        """Pareto-front flags of the rows of ``values`` [n, M] (sign-normalised: every objective minimised): True
+        where no row is <= the row everywhere and < somewhere.  Leaves the history and the suggestion state of
+        this engine unchanged (tpe_pareto_front)."""
+        v = _f64(values)
+        if v.ndim != 2:
+            raise ValueError(f"values must be [n, n_objectives], got shape {v.shape}")
+        out = np.empty(v.shape[0], dtype=np.uint8)
+        self._check(self._lib.tpe_pareto_front(self._h, _ptr(v), v.shape[0], v.shape[1], _ptr(out)))
+        return out.view(bool)
+
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:
         below = np.empty(self._info[1], dtype=np.int64)
