@@ -37,7 +37,8 @@ extern "C" {
 /* 6: + tpe_set_kernel_shard / tpe_sample_and_partial / tpe_finish_from_partials */
 /* 7: + tpe_hypervolume_history */
 /* 8: + tpe_pareto_front */
-#define TPE_ABI_VERSION 8
+/* 9: + tpe_fanova_variances */
+#define TPE_ABI_VERSION 9
 
 enum {
   TPE_OK = 0,
@@ -272,6 +273,25 @@ int tpe_hypervolume_history(tpe_ctx* ctx, const double* values, const uint8_t* f
  * +-inf are ordinary values).  1 <= n_objectives <= 16; NaN in values is TPE_E_INVALID.  Uses its own device memory
  * and leaves the context's history and suggestion state alone. */
 int tpe_pareto_front(tpe_ctx* ctx, const double* values, int64_t n, int32_t n_objectives, uint8_t* on_front);
+/* fANOVA variances of a fitted random forest (replaces the per-tree work of optuna/importance/_fanova: the
+ * _FanovaTree precomputation, _tree.py:144-236, its variance, :33-45, and get_marginal_variance with its tree walk per
+ * grid cell, :47-142, as _Fanova.fit / _compute_variances, _fanova.py:53-108, call them).
+ * Trees t = 0..n_trees-1 are the nodes [node_offsets[t], node_offsets[t+1]) of the concatenated arrays left, right
+ * (children, indices within the tree), feature (< 0: leaf), threshold (x <= threshold goes left) and value (the
+ * node's prediction), as sklearn's tree_.children_left / children_right / feature / threshold / value[:, 0, 0].
+ * bounds [n_features, 2]: the search space of the raw features.  Parameter p is the raw features
+ * raw_features[param_offsets[p] .. param_offsets[p+1]) (one column, or the one-hot columns of a categorical).
+ * Out: tree_variance [n_trees] and marginal_variance [n_params, n_trees] (unclipped).
+ * TPE_E_INVALID: a child index not in (parent, tree size), a node with no or two parents, an internal node's feature
+ * >= n_features, a NaN threshold or one outside its feature's bounds, a raw feature out of range or in two
+ * parameters, and a parameter whose grid (the product of its columns' midpoint counts) exceeds 2^20 cells in some
+ * tree -- the reference would walk that tree 2^20 times per parameter; this is the one input it accepts that is
+ * refused here.  TPE_E_NOMEM when the device memory runs out.  Uses its own device memory and leaves the context's
+ * history and suggestion state alone. */
+int tpe_fanova_variances(tpe_ctx* ctx, int32_t n_trees, const int64_t* node_offsets, const int32_t* left,
+                         const int32_t* right, const int32_t* feature, const double* threshold, const double* value,
+                         int32_t n_features, const double* bounds, int32_t n_params, const int32_t* param_offsets,
+                         const int32_t* raw_features, double* tree_variance, double* marginal_variance);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

@@ -7,7 +7,7 @@ sm_90a CUDA through a C ABI (include/optuna_b200_tpe.h) bound with ctypes.
 from .engine import ParamSpec, TPEEngine  # noqa: F401
 
 __all__ = ["ParamSpec", "TPEEngine", "B200TPESampler", "hypervolume_history", "plot_hypervolume_history",
-           "best_trials", "pareto_front_info", "plot_pareto_front"]
+           "best_trials", "pareto_front_info", "plot_pareto_front", "FanovaImportanceEvaluator"]
 
 
 def __getattr__(name):
@@ -18,4 +18,7 @@ def __getattr__(name):
                 "plot_pareto_front"):
         from . import analysis
         return getattr(analysis, name)
+    if name == "FanovaImportanceEvaluator":
+        from .importance import FanovaImportanceEvaluator
+        return FanovaImportanceEvaluator
     raise AttributeError(name)

@@ -72,6 +72,8 @@ SYMBOLS = {
     "tpe_get_mo_weights": (C.c_int, [_P, _P]),
     "tpe_hypervolume_history": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int32, _P, _P]),
     "tpe_pareto_front": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P]),
+    "tpe_fanova_variances": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, _P, C.c_int32, _P, _P,
+                                       _P, _P]),
     "tpe_get_candidates": (C.c_int, [_P, _P, _P, _P]),
     "tpe_logpdf": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P]),
     "tpe_last_timing": (C.c_int, [_P, _P, _P]),
@@ -82,7 +84,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 8  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 9  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

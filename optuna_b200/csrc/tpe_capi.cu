@@ -21,6 +21,7 @@
 #include "tpe_motpe_kernels.cuh"
 #include "tpe_hvhist.cuh"
 #include "tpe_pareto.cuh"
+#include "tpe_fanova.cuh"
 #include "tpe_uni.cuh"
 #include "tpe_mixed.cuh"
 #include "tpe_tcscreen.cuh"
@@ -1906,6 +1907,249 @@ int pareto_front_run(tpe_ctx* ctx, const double* values, int n, int M, uint8_t* 
   return TPE_OK;
 }
 
+// ---- fANOVA variances (tpe_fanova.cuh) -----------------------------------------------------------
+// Device memory of one tpe_fanova_variances call, released when it returns: nothing a suggestion reads is touched.
+struct FaScratch {
+  DevBuf off, left, right, feat, thr, val, parent, tree_of, bounds, fparam, po, cols, stat, mask, tvar, mvar;
+  DevBuf box, lvl, key1, key2, k2s, key, idx, work, so, ebuf, mp, sz, K, acc_off, acc;
+  ~FaScratch() {
+    for (DevBuf* b : {&off, &left, &right, &feat, &thr, &val, &parent, &tree_of, &bounds, &fparam, &po, &cols, &stat,
+                      &mask, &tvar, &mvar, &box, &lvl, &key1, &key2, &k2s, &key, &idx, &work, &so, &ebuf, &mp, &sz,
+                      &K, &acc_off, &acc})
+      b->release();
+  }
+};
+
+constexpr size_t kFaBoxBudget = (size_t)1 << 30;   // bytes of per-node boxes (nodes x F x 16) per chunk of trees
+
+// The validated forest: global child / parent indices (-1: none), the tree and depth of every node.
+struct FaForest {
+  std::vector<int32_t> left, right, parent, tree_of, depth;
+};
+
+// The host checks of tpe_fanova_variances; fills fo.  Returns TPE_OK or TPE_E_INVALID (message in ctx).
+int fanova_validate(tpe_ctx* ctx, int T, const int64_t* off, const int32_t* left, const int32_t* right,
+                    const int32_t* feature, const double* thr, int F, const double* bounds, int n_params,
+                    const int32_t* po, const int32_t* cols, FaForest& fo) {
+  if (off[0] != 0) return fail(ctx, TPE_E_INVALID, "node_offsets[0] must be 0");
+  for (int t = 0; t < T; ++t)
+    if (off[t + 1] <= off[t]) return fail(ctx, TPE_E_INVALID, "tree %d has no nodes", t);
+  const int64_t N = off[T];
+  if (N >= (1ll << 31) - 1) return fail(ctx, TPE_E_INVALID, "too many nodes (%lld)", (long long)N);
+  for (int f = 0; f < F; ++f)
+    if (!(bounds[2 * f] <= bounds[2 * f + 1])) return fail(ctx, TPE_E_INVALID, "bad bounds of feature %d", f);
+  if (po[0] != 0) return fail(ctx, TPE_E_INVALID, "param_offsets[0] must be 0");
+  std::vector<uint8_t> used((size_t)F, 0);
+  for (int p = 0; p < n_params; ++p) {
+    if (po[p + 1] <= po[p]) return fail(ctx, TPE_E_INVALID, "parameter %d has no raw features", p);
+    for (int j = po[p]; j < po[p + 1]; ++j) {
+      if (cols[j] < 0 || cols[j] >= F || used[cols[j]])
+        return fail(ctx, TPE_E_INVALID, "raw feature %d of parameter %d is out of range or repeated", cols[j], p);
+      used[cols[j]] = 1;
+    }
+  }
+  fo.left.assign((size_t)N, -1);
+  fo.right.assign((size_t)N, -1);
+  fo.parent.assign((size_t)N, -1);
+  fo.tree_of.resize((size_t)N);
+  fo.depth.assign((size_t)N, 0);
+  for (int t = 0; t < T; ++t) {
+    const int64_t a = off[t], n_t = off[t + 1] - a;
+    for (int64_t i = 0; i < n_t; ++i) {
+      const int64_t g = a + i;
+      fo.tree_of[g] = t;
+      const int f = feature[g];
+      if (f < 0) continue;
+      if (f >= F) return fail(ctx, TPE_E_INVALID, "tree %d node %lld splits on feature %d >= %d", t, (long long)i, f, F);
+      const double th = thr[g];
+      if (std::isnan(th) || th < bounds[2 * f] || th > bounds[2 * f + 1])
+        return fail(ctx, TPE_E_INVALID, "tree %d node %lld: threshold is NaN or outside its feature's bounds", t,
+                    (long long)i);
+      for (int32_t c : {left[g], right[g]}) {
+        if (c <= i || c >= n_t)
+          return fail(ctx, TPE_E_INVALID, "tree %d node %lld: child %d is not in (%lld, %lld)", t, (long long)i, c,
+                      (long long)i, (long long)n_t);
+        if (fo.parent[a + c] >= 0)
+          return fail(ctx, TPE_E_INVALID, "tree %d node %d has two parents", t, c);
+        fo.parent[a + c] = (int32_t)g;
+        fo.depth[a + c] = fo.depth[g] + 1;
+      }
+      if (left[g] == right[g]) return fail(ctx, TPE_E_INVALID, "tree %d node %lld: equal children", t, (long long)i);
+      fo.left[g] = (int32_t)(a + left[g]);
+      fo.right[g] = (int32_t)(a + right[g]);
+    }
+    for (int64_t i = 1; i < n_t; ++i)
+      if (fo.parent[a + i] < 0) return fail(ctx, TPE_E_INVALID, "tree %d node %lld has no parent", t, (long long)i);
+  }
+  return TPE_OK;
+}
+
+int fanova_run(tpe_ctx* ctx, int T, const int64_t* off, const FaForest& fo, const int32_t* feature, const double* thr,
+               const double* value, int F, const double* bounds, int n_params, const int32_t* po,
+               const int32_t* cols, double* tree_var, double* marginal_var) {
+  cudaStream_t st = ctx->stream;
+  FaScratch b;
+  const int64_t N = off[T];
+  const int n_cols = po[n_params];
+  const int n_words = std::max(1, (n_params + 63) / 64);
+  std::vector<int32_t> fparam((size_t)F, -1);
+  for (int p = 0; p < n_params; ++p)
+    for (int j = po[p]; j < po[p + 1]; ++j) fparam[cols[j]] = p;
+  auto up = [&](DevBuf& d, const void* h, size_t bytes) -> cudaError_t {
+    cudaError_t e = d.ensure(std::max<size_t>(bytes, 8));
+    if (e == cudaSuccess && bytes) e = cudaMemcpyAsync(d.p, h, bytes, cudaMemcpyHostToDevice, st);
+    return e;
+  };
+  CU(up(b.off, off, (size_t)(T + 1) * 8));
+  CU(up(b.left, fo.left.data(), (size_t)N * 4));
+  CU(up(b.right, fo.right.data(), (size_t)N * 4));
+  CU(up(b.parent, fo.parent.data(), (size_t)N * 4));
+  CU(up(b.tree_of, fo.tree_of.data(), (size_t)N * 4));
+  CU(up(b.feat, feature, (size_t)N * 4));
+  CU(up(b.thr, thr, (size_t)N * 8));
+  CU(up(b.val, value, (size_t)N * 8));
+  CU(up(b.bounds, bounds, (size_t)F * 16));
+  CU(up(b.fparam, fparam.data(), (size_t)F * 4));
+  CU(up(b.po, po, (size_t)(n_params + 1) * 4));
+  CU(up(b.cols, cols, (size_t)n_cols * 4));
+  CU(b.stat.ensure((size_t)N * 16));
+  CU(b.mask.ensure((size_t)N * n_words * 8));
+  CU(b.tvar.ensure((size_t)T * 8));
+  CU(b.mvar.ensure((size_t)std::max(1, n_params) * T * 8));
+  CU(b.work.ensure(sizeof(SortWork)));
+  const int32_t* d_feat = b.feat.as<int32_t>();
+  const double* d_thr = b.thr.as<double>();
+  const double2* d_bounds = b.bounds.as<double2>();
+  std::vector<int32_t> lvl;
+  std::vector<int64_t> lvl_off, so;
+  std::vector<int32_t> Kh;
+  std::vector<int64_t> acc_off;
+  for (int t0 = 0; t0 < T;) {
+    // 0. a chunk [t0, t1) of trees whose boxes fit kFaBoxBudget (at least one tree)
+    int t1 = t0 + 1;
+    while (t1 < T && (size_t)(off[t1 + 1] - off[t0]) * F * 16 <= kFaBoxBudget) ++t1;
+    const int Tc = t1 - t0, n_seg = Tc * F;
+    const int64_t base = off[t0];
+    const int cnt = (int)(off[t1] - base);
+    // nodes by depth (counting sort) and internal nodes per (tree, feature) segment
+    int max_d = 0;
+    for (int i = 0; i < cnt; ++i) max_d = std::max(max_d, fo.depth[base + i]);
+    lvl_off.assign((size_t)max_d + 2, 0);
+    so.assign((size_t)n_seg + 1, 0);
+    for (int i = 0; i < cnt; ++i) {
+      ++lvl_off[fo.depth[base + i] + 1];
+      if (feature[base + i] >= 0) ++so[(size_t)(fo.tree_of[base + i] - t0) * F + feature[base + i] + 1];
+    }
+    for (int d = 0; d <= max_d; ++d) lvl_off[d + 1] += lvl_off[d];
+    for (int s = 0; s < n_seg; ++s) so[s + 1] += so[s];
+    lvl.resize((size_t)cnt);
+    {
+      std::vector<int64_t> at(lvl_off.begin(), lvl_off.end() - 1);
+      for (int i = 0; i < cnt; ++i) lvl[at[fo.depth[base + i]]++] = (int32_t)(base + i);
+    }
+    CU(up(b.lvl, lvl.data(), (size_t)cnt * 4));
+    CU(up(b.so, so.data(), (size_t)(n_seg + 1) * 8));
+    CU(b.box.ensure((size_t)cnt * F * 16));
+    // 1-2. boxes top-down, leaves, statistics and subtree parameter masks bottom-up
+    for (int d = 0; d <= max_d; ++d) {
+      const int n_l = (int)(lvl_off[d + 1] - lvl_off[d]);
+      const int64_t work = (int64_t)n_l * F;
+      k_fa_down<<<(unsigned)((work + 255) / 256), 256, 0, st>>>(b.lvl.as<int32_t>() + lvl_off[d], n_l, base,
+                                                               b.parent.as<int32_t>(), b.left.as<int32_t>(), d_feat,
+                                                               d_thr, d_bounds, F, b.box.as<double2>());
+    }
+    k_fa_leaf<<<(cnt + 255) / 256, 256, 0, st>>>(base, cnt, d_feat, b.val.as<double>(), b.box.as<double2>(), F, n_words,
+                                                  b.stat.as<double2>(), b.mask.as<uint64_t>());
+    for (int d = max_d; d >= 0; --d) {
+      const int n_l = (int)(lvl_off[d + 1] - lvl_off[d]);
+      k_fa_up<<<(n_l + 255) / 256, 256, 0, st>>>(b.lvl.as<int32_t>() + lvl_off[d], n_l, b.left.as<int32_t>(),
+                                                 b.right.as<int32_t>(), d_feat, b.fparam.as<int32_t>(), n_words,
+                                                 b.stat.as<double2>(), b.mask.as<uint64_t>());
+    }
+    CU(cudaGetLastError());
+    // 3. tree variances
+    k_fa_tree_var<<<Tc, kFaThreads, 0, st>>>(b.off.as<int64_t>(), t0, d_feat, b.stat.as<double2>(),
+                                             b.tvar.as<double>());
+    // 4. (tree, feature, threshold) order by two stable radix sorts, then the midpoints of every segment
+    for (DevBuf* x : {&b.key1, &b.key2, &b.k2s}) CU(x->ensure((size_t)cnt * 8));
+    CU(b.key.ensure((size_t)cnt * 16));
+    CU(b.idx.ensure((size_t)cnt * 16));
+    k_fa_keys<<<(cnt + 255) / 256, 256, 0, st>>>(base, cnt, t0, n_seg, b.tree_of.as<int32_t>(), d_feat, d_thr, F,
+                                                  b.key1.as<double>(), b.key2.as<double>());
+    CU(cudaGetLastError());
+    int32_t* order1 = b.idx.as<int32_t>();
+    int32_t* order2 = order1 + cnt;
+    auto sort = [&](const double* keys, int32_t* order) -> cudaError_t {
+      int32_t pc = 1;
+      int j_col = 0, n_i = cnt;
+      uint64_t* ka = b.key.as<uint64_t>();
+      uint64_t* kb = ka + cnt;
+      int32_t* ia = order2 + cnt;
+      int32_t* ib = ia + cnt;
+      SortWork* wk = b.work.as<SortWork>();
+      const int* run_flag = nullptr;
+      void* args[] = {&keys, &pc, &j_col, &n_i, &ka, &kb, &ia, &ib, &wk, &order, &run_flag};
+      int G = std::max(1, std::min(std::min(ctx->sm_count, 160), (cnt + 1023) / 1024));
+      if (ctx->sort_cta_cap > 0) G = std::min(G, ctx->sort_cta_cap);
+      return cudaLaunchCooperativeKernel((const void*)k_radix_sort_coop, dim3(G), dim3(512), args, 0, st);
+    };
+    CU(sort(b.key1.as<double>(), order1));
+    k_fa_gather<<<(cnt + 255) / 256, 256, 0, st>>>(order1, cnt, b.key2.as<double>(), b.k2s.as<double>());
+    CU(sort(b.k2s.as<double>(), order2));
+    const int64_t n_int = so[n_seg];
+    CU(b.ebuf.ensure((size_t)(n_int + 2 * n_seg) * 8));
+    CU(b.mp.ensure((size_t)(n_int + n_seg) * 8));
+    CU(b.sz.ensure((size_t)(n_int + n_seg) * 8));
+    CU(b.K.ensure((size_t)n_seg * 4));
+    k_fa_midpoints<<<n_seg, 1024, 0, st>>>(base, order1, order2, b.so.as<int64_t>(), d_thr, d_bounds, F,
+                                           b.ebuf.as<double>(), b.mp.as<double>(), b.sz.as<double>(),
+                                           b.K.as<int32_t>());
+    CU(cudaGetLastError());
+    Kh.resize((size_t)n_seg);
+    CU(cudaMemcpyAsync(Kh.data(), b.K.p, (size_t)n_seg * 4, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (n_params == 0) {
+      t0 = t1;
+      continue;
+    }
+    // 5. accumulator of every (tree, parameter): a segment tree for one column, the grid for several
+    acc_off.assign((size_t)Tc * n_params + 1, 0);
+    for (int tl = 0; tl < Tc; ++tl)
+      for (int p = 0; p < n_params; ++p) {
+        int64_t cells = 1;
+        for (int j = po[p]; j < po[p + 1] && cells <= kFaMaxCells; ++j) cells *= Kh[(size_t)tl * F + cols[j]];
+        if (cells > kFaMaxCells)
+          return fail(ctx, TPE_E_INVALID,
+                      "parameter %d: tree %d splits its %d raw features into more than 2^20 grid cells", p, t0 + tl,
+                      po[p + 1] - po[p]);
+        int64_t sz_acc = cells;
+        if (po[p + 1] - po[p] == 1) {
+          int64_t P = 1;
+          while (P < cells) P <<= 1;
+          sz_acc = 2 * P;
+        }
+        acc_off[(size_t)tl * n_params + p + 1] = acc_off[(size_t)tl * n_params + p] + sz_acc;
+      }
+    CU(up(b.acc_off, acc_off.data(), acc_off.size() * 8));
+    CU(b.acc.ensure((size_t)acc_off.back() * 16));
+    CU(cudaMemsetAsync(b.acc.p, 0, (size_t)acc_off.back() * 16, st));
+    k_fa_marginal<<<dim3((unsigned)n_params, (unsigned)Tc), kFaThreads, 0, st>>>(
+        b.off.as<int64_t>(), t0, base, n_params, b.po.as<int32_t>(), b.cols.as<int32_t>(), b.parent.as<int32_t>(),
+        b.stat.as<double2>(), b.mask.as<uint64_t>(), n_words, b.box.as<double2>(), F, b.so.as<int64_t>(),
+        b.mp.as<double>(), b.sz.as<double>(), b.K.as<int32_t>(), b.acc_off.as<int64_t>(), b.acc.as<double2>(),
+        b.mvar.as<double>(), T);
+    CU(cudaGetLastError());
+    // the next chunk overwrites the host vectors the pending copies read
+    CU(cudaStreamSynchronize(st));
+    t0 = t1;
+  }
+  CU(cudaMemcpyAsync(tree_var, b.tvar.p, (size_t)T * 8, cudaMemcpyDeviceToHost, st));
+  if (n_params > 0)
+    CU(cudaMemcpyAsync(marginal_var, b.mvar.p, (size_t)n_params * T * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
 
 // =================================================================================================
 extern "C" {
@@ -2182,6 +2426,27 @@ int tpe_pareto_front(tpe_ctx* ctx, const double* values, int64_t n, int32_t n_ob
   if (n == 0) return TPE_OK;
   if (set_device(ctx, false)) return TPE_E_CUDA;
   return pareto_front_run(ctx, values, (int)n, M, on_front);
+}
+
+int tpe_fanova_variances(tpe_ctx* ctx, int32_t n_trees, const int64_t* node_offsets, const int32_t* left,
+                         const int32_t* right, const int32_t* feature, const double* threshold, const double* value,
+                         int32_t n_features, const double* bounds, int32_t n_params, const int32_t* param_offsets,
+                         const int32_t* raw_features, double* tree_variance, double* marginal_variance) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (n_trees < 1 || n_features < 1 || n_params < 0)
+    return fail(ctx, TPE_E_INVALID, "bad sizes (n_trees %d, n_features %d, n_params %d)", n_trees, n_features,
+                n_params);
+  if (!node_offsets || !left || !right || !feature || !threshold || !value || !bounds || !param_offsets ||
+      (n_params > 0 && (!raw_features || !marginal_variance)) || !tree_variance)
+    return fail(ctx, TPE_E_INVALID, "bad fANOVA arguments");
+  FaForest fo;
+  const int rc = fanova_validate(ctx, n_trees, node_offsets, left, right, feature, threshold, n_features, bounds,
+                                 n_params, param_offsets, raw_features, fo);
+  if (rc != TPE_OK) return rc;
+  if (set_device(ctx, false)) return TPE_E_CUDA;
+  return fanova_run(ctx, n_trees, node_offsets, fo, feature, threshold, value, n_features, bounds, n_params,
+                    param_offsets, raw_features, tree_variance, marginal_variance);
 }
 
 int64_t tpe_history_size(tpe_ctx* ctx) { return ctx ? ctx->N : -1; }

@@ -391,6 +391,32 @@ class TPEEngine:
         self._check(self._lib.tpe_pareto_front(self._h, _ptr(v), v.shape[0], v.shape[1], _ptr(out)))
         return out.view(bool)
 
+    def fanova_variances(self, node_offsets, left, right, feature, threshold, value, bounds, param_offsets,
+                         raw_features) -> tuple[np.ndarray, np.ndarray]:
+        """fANOVA variances of a forest (tpe_fanova_variances): ``(tree_variance [T], marginal_variance
+        [n_params, T])``.  Tree t is the nodes ``[node_offsets[t], node_offsets[t + 1])`` of the concatenated
+        sklearn arrays (children indexed within their tree); parameter p is the raw features
+        ``raw_features[param_offsets[p]:param_offsets[p + 1]]``.  Leaves the history and the suggestion state of
+        this engine unchanged."""
+        off = np.ascontiguousarray(node_offsets, dtype=np.int64)
+        i32 = [np.ascontiguousarray(a, dtype=np.int32) for a in (left, right, feature)]
+        thr, val = _f64(threshold), _f64(value)
+        bnd = _f64(bounds)
+        po = np.ascontiguousarray(param_offsets, dtype=np.int32)
+        cols = np.ascontiguousarray(raw_features, dtype=np.int32)
+        T, n_params = off.size - 1, po.size - 1
+        if bnd.ndim != 2 or bnd.shape[1] != 2:
+            raise ValueError(f"bounds must be [n_features, 2], got shape {bnd.shape}")
+        n = int(off[-1]) if off.size else 0
+        if T < 1 or any(a.shape != (n,) for a in (*i32, thr, val)) or n_params < 0 or cols.size != int(po[-1]):
+            raise ValueError("inconsistent fANOVA forest arrays")
+        tree_var = np.empty(T)
+        marg = np.empty((max(n_params, 0), T))
+        self._check(self._lib.tpe_fanova_variances(self._h, T, _ptr(off), *(_ptr(a) for a in i32), _ptr(thr),
+                                                   _ptr(val), bnd.shape[0], _ptr(bnd), n_params, _ptr(po),
+                                                   _ptr(cols), _ptr(tree_var), _ptr(marg)))
+        return tree_var, marg
+
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:
         below = np.empty(self._info[1], dtype=np.int64)
