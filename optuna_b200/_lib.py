@@ -9,7 +9,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# TPE_LAB=1 loads the lab build (experimental kernels selectable by TPE_MMA_VARIANT etc., see DESIGN.md section 6)
+# TPE_LAB=1 loads the lab build (experimental kernels selectable by TPE_MMA_LAB etc., see DESIGN.md section 6)
 LIB_PATH = os.path.join(_HERE, "libtpe_b200_lab.so" if os.environ.get("TPE_LAB") == "1" else "libtpe_b200.so")
 
 TPE_OK, TPE_E_INVALID, TPE_E_CUDA, TPE_E_STATE, TPE_E_NOMEM = 0, -1, -2, -3, -4

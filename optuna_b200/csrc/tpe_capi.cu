@@ -310,7 +310,7 @@ struct FastInst {
 constexpr int kMmaKPad = 32;  // kernels are padded to 8 * KG (KG <= 4)
 template <int PB, int M, int KG, int NT, int TK, int ST, int MINB, int DBG = 0>
 struct MmaInst {
-  static constexpr size_t smem = (size_t)ST * TK * PB * 8 + (size_t)ST * TK * 8 + (size_t)ST * 16;
+  static constexpr size_t smem = MmaSmem<PB, M, KG, NT, TK, ST, MINB>::bytes;   // TMA stages + near-term ring
   static void launch(dim3 grid, size_t sm, cudaStream_t st, const void* tab, const double* cst, int64_t Kf,
                      const double2* colprm, const double* xT, int64_t ct_stride, int64_t kps, double skip,
                      double2* part, unsigned long long* gmax) {
@@ -343,9 +343,11 @@ struct MmaInst {
 //   pairs of runs (the means of one tiling spread by 0.003 ms, the gap is 0.037 ms).
 // Small path (one ask of 24 candidates): m8n8k4 stays at P <= 32 (14-30 % faster there).  At P = 64 m16n8k8 wins
 // since the steps are software-pipelined: 0.061 against 0.065 ms (H100 SXM, 400 W).
+// The big path at P = 8 and 16 runs 2 TMA stages of the same tile instead of 3, so that the near-term ring
+// (MmaSmem) fits beside them at 2 CTAs per SM.
 //                                   PB M KG  NT   TK ST MINB
 const FastCfg kMmaBig[] = {
-    MmaInst<8, 1, 4, 256, 512, 3, 2>::cfg(), MmaInst<16, 2, 2, 256, 256, 3, 2>::cfg(),
+    MmaInst<8, 1, 4, 256, 512, 2, 2>::cfg(), MmaInst<16, 2, 2, 256, 256, 2, 2>::cfg(),
     MmaInst<32, 2, 1, 256, 128, 2, 2>::cfg(), MmaInst<64, 2, 2, 256, 64, 3, 1>::cfg(),
 };
 const FastCfg kMmaSmall[] = {
@@ -353,15 +355,10 @@ const FastCfg kMmaSmall[] = {
     MmaInst<32, 1, 4, 64, 128, 3, 4>::cfg(), MmaInst<64, 2, 2, 64, 64, 3, 3>::cfg(),
 };
 #ifdef TPE_LAB
-const FastCfg kMma32Variants[] = {
-    MmaInst<32, 1, 4, 256, 128, 3, 2>::cfg(), MmaInst<32, 1, 2, 256, 128, 3, 2>::cfg(),
-    MmaInst<32, 1, 1, 512, 128, 3, 2>::cfg(), MmaInst<32, 1, 2, 256, 128, 2, 3>::cfg(),
-    MmaInst<32, 1, 2, 512, 128, 3, 2>::cfg(), MmaInst<32, 1, 2, 512, 128, 3, 2, 1>::cfg(),
-    MmaInst<32, 1, 2, 512, 128, 3, 2, 2>::cfg(), MmaInst<32, 1, 4, 256, 128, 3, 2, 1>::cfg(),
-};
 // Tilings for every width, big and small path, selected by TPE_MMA_LAB=<index> when the width matches
 // (tools/tune_mma.py); DBG = 1 / 2 time the mma + TMA floor and the classification + far tier alone, DBG = 4 the mma +
-// TMA floor without the per-tile exchange of maxima (sync_global).
+// TMA floor without the per-tile exchange of maxima (sync_global), DBG = 5 is the full kernel with the near-term
+// counters (g_mma_lab_count, read by tpe_lab_mma_counters).
 //                                   PB M KG  NT   TK ST MINB DBG
 const FastCfg kMmaLab[] = {
     MmaInst<32, 1, 2, 256, 128, 2, 3, 1>::cfg(),  //  0
@@ -379,14 +376,14 @@ const FastCfg kMmaLab[] = {
     MmaInst<32, 2, 2, 64, 128, 3, 4>::cfg(),      // 12  small
     MmaInst<32, 2, 1, 64, 128, 3, 4>::cfg(),      // 13  small
     MmaInst<32, 2, 4, 64, 128, 3, 2>::cfg(),      // 14  small
-    MmaInst<8, 2, 2, 256, 512, 3, 2>::cfg(),      // 15
-    MmaInst<8, 2, 4, 256, 512, 3, 2>::cfg(),      // 16
-    MmaInst<8, 2, 2, 256, 512, 3, 3>::cfg(),      // 17
+    MmaInst<8, 2, 2, 256, 512, 2, 2>::cfg(),      // 15
+    MmaInst<8, 2, 4, 256, 512, 2, 2>::cfg(),      // 16
+    MmaInst<8, 1, 4, 256, 256, 3, 2>::cfg(),      // 17
     MmaInst<8, 2, 2, 64, 512, 3, 4>::cfg(),       // 18  small
-    MmaInst<8, 2, 4, 64, 512, 3, 4>::cfg(),       // 19  small
-    MmaInst<16, 2, 2, 256, 256, 3, 2>::cfg(),     // 20
-    MmaInst<16, 2, 4, 256, 256, 3, 2>::cfg(),     // 21
-    MmaInst<16, 2, 2, 256, 256, 2, 3>::cfg(),     // 22
+    MmaInst<8, 2, 4, 64, 256, 2, 4>::cfg(),       // 19  small
+    MmaInst<16, 2, 2, 256, 128, 3, 2>::cfg(),     // 20
+    MmaInst<16, 2, 4, 256, 256, 2, 2>::cfg(),     // 21
+    MmaInst<16, 2, 2, 256, 128, 2, 3>::cfg(),     // 22
     MmaInst<16, 2, 2, 64, 256, 3, 4>::cfg(),      // 23  small
     MmaInst<16, 2, 4, 64, 256, 3, 4>::cfg(),      // 24  small
     MmaInst<64, 2, 1, 256, 64, 3, 1>::cfg(),      // 25
@@ -395,6 +392,12 @@ const FastCfg kMmaLab[] = {
     MmaInst<64, 2, 1, 64, 64, 3, 3>::cfg(),       // 28  small
     MmaInst<64, 2, 2, 64, 64, 3, 3>::cfg(),       // 29  small
     MmaInst<32, 2, 1, 256, 128, 2, 2, 4>::cfg(),  // 30  as 7, without the per-tile exchange of maxima
+    MmaInst<16, 2, 2, 256, 256, 2, 2, 5>::cfg(),  // 31  shipped tilings with the near-term counters
+    MmaInst<16, 1, 4, 64, 256, 3, 4, 5>::cfg(),   // 32  small
+    MmaInst<32, 2, 1, 256, 128, 2, 2, 5>::cfg(),  // 33
+    MmaInst<32, 1, 4, 64, 128, 3, 4, 5>::cfg(),   // 34  small
+    MmaInst<64, 2, 2, 256, 64, 3, 1, 5>::cfg(),   // 35
+    MmaInst<64, 2, 2, 64, 64, 3, 3, 5>::cfg(),    // 36  small
 };
 constexpr int kMmaLabN = sizeof(kMmaLab) / sizeof(kMmaLab[0]);
 #endif  // TPE_LAB
@@ -405,10 +408,6 @@ const FastCfg* pick_mma(int pb, int64_t Ct) {
   if (const char* v = getenv("TPE_MMA_LAB")) {
     const int i = atoi(v);
     if (i >= 0 && i < kMmaLabN && kMmaLab[i].pb == pb) return &kMmaLab[i];
-  }
-  if (pb == 32 && !small) {
-    const char* v = getenv("TPE_MMA_VARIANT");
-    if (v && v[0] >= '0' && v[0] <= '7') return &kMma32Variants[v[0] - '0'];
   }
 #endif
   const FastCfg* tabs = small ? kMmaSmall : kMmaBig;
@@ -3483,5 +3482,20 @@ int tpe_probe_fp64_tflops(tpe_ctx* ctx, double* tflops) {
 }
 
 const char* tpe_last_logpdf_kernel(tpe_ctx* ctx) { return ctx ? ctx->last_kernel : "none"; }
+
+#ifdef TPE_LAB
+// lab build only (not in the header): the near-term counters of the DBG = 5 tilings summed since the last call (see
+// g_mma_lab_count), then cleared
+int tpe_lab_mma_counters(tpe_ctx* ctx, unsigned long long* out5) {
+  if (!ctx || !out5) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (set_device(ctx)) return TPE_E_CUDA;
+  CU(cudaStreamSynchronize(ctx->stream));
+  CU(cudaMemcpyFromSymbol(out5, g_mma_lab_count, 5 * sizeof(unsigned long long)));
+  const unsigned long long zero[5] = {0, 0, 0, 0, 0};
+  CU(cudaMemcpyToSymbol(g_mma_lab_count, zero, sizeof(zero)));
+  return TPE_OK;
+}
+#endif  // TPE_LAB
 
 }  // extern "C"

@@ -1500,16 +1500,23 @@ __device__ __forceinline__ double uni_exp(double x, const double* __restrict__ t
 // kRefMove above it, so R <= base <= R + kRefMove at all times.  Hence a far term has -skip < L - R <= kRefMove -
 // tnear (|L - R| < 64 for any K <= e^34), a near term e^(L - R) <= e^kRefMove, and the exact terms need no running
 // max: they are independent exponentials, and a rise of base costs no rescale.
+// Near terms are parked as raw L in a per-(lane, candidate group) ring of D slots in shared memory, slot i at
+// ring[i * RS] (slot-major, so a warp's store or load is conflict-free whatever each lane's count): a near term is
+// stored with a predicated store and no branch, and one warp vote per step decides whether to flush (MmaSmem).
 constexpr double kRefMove = 48.0;
+__device__ __forceinline__ unsigned long long ld_relaxed_gpu(const unsigned long long* p) {
+  unsigned long long v;
+  asm volatile("ld.relaxed.gpu.global.u64 %0, [%1];" : "=l"(v) : "l"(p));
+  return v;
+}
 struct LseRef {
   double R, s, base;     // reference, sum of e^(L - R), classification base
-  double b0, b1, b2, b3; // parked near terms
   float ffar;            // current fp32 run of far terms, relative to R
   float thn;             // near threshold on fl(L - R): fl(base - R) - tnear (far: - skip)
-  int cnt;
-  __device__ __forceinline__ void init() {
-    R = -INFINITY; s = 0.0; base = -INFINITY; b0 = b1 = b2 = b3 = 0.0;
-    ffar = 0.0f; thn = -INFINITY; cnt = 0;   // cold: every finite term is near
+  unsigned wp;           // shared-memory address of the next free ring slot: slot0 + (parked terms) * RS * 8
+  __device__ __forceinline__ void init(unsigned slot0) {
+    R = -INFINITY; s = 0.0; base = -INFINITY;
+    ffar = 0.0f; thn = -INFINITY; wp = slot0;   // cold: every finite term is near
   }
   // base := nb (>= base); R follows when nb is more than kRefMove above it (also the cold start, R = -inf: s and the
   // far run are 0 then).  Executed by the whole warp together.
@@ -1525,64 +1532,64 @@ struct LseRef {
     const float d = __double2float_rn(base - R);   // R = -inf only while base = -inf: stay cold
     thn = (R == -INFINITY) ? -INFINITY : d - tnear;
   }
-  // fold the parked terms (executed by the whole warp together): base first, then up to 4 independent exps
-  __device__ __forceinline__ void flush(float tnear, const double* e64) {
-    const bool v0 = cnt > 0, v1 = cnt > 1, v2 = cnt > 2, v3 = cnt > 3;
+  // fold the parked terms (executed by the whole warp together): base first (to the largest parked term, so that
+  // e^(L - R) <= e^kRefMove), then independent exps over the slots any lane of the warp has filled
+  template <int RS>
+  __device__ __forceinline__ void flush(const double* ring, float tnear, const double* e64) {
+    const unsigned slot0 = (unsigned)__cvta_generic_to_shared(ring);
+    const int cnt = parked<RS>(slot0);
+    const int n = __reduce_max_sync(0xffffffffu, cnt);
     double nb = base;
-    nb = (v0 && b0 > nb) ? b0 : nb;
-    nb = (v1 && b1 > nb) ? b1 : nb;
-    nb = (v2 && b2 > nb) ? b2 : nb;
-    nb = (v3 && b3 > nb) ? b3 : nb;
+    for (int i = 0; i < n; ++i) {
+      const double v = ring[i * RS];
+      nb = (i < cnt && v > nb) ? v : nb;
+    }
     rebase(nb, tnear, e64);
-    // stale slots may hold anything: selected away, never multiplied
-    const double e0 = uni_exp(fmax(b0 - R, -700.0), e64), e1 = uni_exp(fmax(b1 - R, -700.0), e64);
-    const double e2 = uni_exp(fmax(b2 - R, -700.0), e64), e3 = uni_exp(fmax(b3 - R, -700.0), e64);
-    s += ((v0 ? e0 : 0.0) + (v1 ? e1 : 0.0)) + ((v2 ? e2 : 0.0) + (v3 ? e3 : 0.0));
-    cnt = 0;
+    double sum = 0.0;
+    for (int i = 0; i < n; ++i) {   // slots >= cnt may hold anything: selected away, never multiplied
+      const double e = uni_exp(fmax(ring[i * RS] - R, -700.0), e64);
+      sum += (i < cnt) ? e : 0.0;
+    }
+    s += sum;
+    wp = slot0;
   }
+  // park L in the next free slot if it is near: a predicated store (written in PTX: the compiler turns `if (near)`
+  // into a branch), no vote
+  template <int RS>
+  __device__ __forceinline__ void park(double L, bool near) {
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.u32 p, %2, 0;\n\t@p st.shared.f64 [%0], %1;\n\t}"
+                 :: "r"(wp), "d"(L), "r"((unsigned)near) : "memory");
+    wp += near ? RS * 8 : 0;
+  }
+  // terms parked in the ring starting at slot0
+  template <int RS>
+  __device__ __forceinline__ int parked(unsigned slot0) const { return (int)((wp - slot0) / (RS * 8)); }
   __device__ __forceinline__ void roll() {  // bounds the length of the fp32 runs (once per tile)
     s += (double)ffar;
     ffar = 0.0f;
   }
   // Publish base in `slot` (ordered-integer atomicMax) and adopt a larger one published by the k-splits and lanes
-  // that share the candidate.  Any published value is some kernel's L, hence <= the true max.
-  __device__ __forceinline__ void sync_global(unsigned long long* slot, float tnear, const double* e64) {
-    const double seen = from_order_bits(*reinterpret_cast<volatile unsigned long long*>(slot));
+  // that share the candidate.  Any published value is some kernel's L, hence <= the true max.  `pend` holds the
+  // slot as read at the previous exchange; the read for the next one is issued here, so its L2 round trip overlaps
+  // the tile instead of stalling the warp.
+  __device__ __forceinline__ void sync_global(unsigned long long* slot, unsigned long long& pend, float tnear,
+                                              const double* e64) {
+    const double seen = from_order_bits(pend);
+    pend = ld_relaxed_gpu(slot);
     if (base > seen) atomicMax(slot, static_cast<unsigned long long>(order_bits(base)));
     if (__any_sync(0xffffffffu, seen > base)) rebase(fmax(base, seen), tnear, e64);
   }
-  __device__ __forceinline__ void park(double L, bool near, float tnear, const double* e64) {
-    b3 = near ? b2 : b3;
-    b2 = near ? b1 : b2;
-    b1 = near ? b0 : b1;
-    b0 = near ? L : b0;
-    cnt += near ? 1 : 0;
-    if (__any_sync(0xffffffffu, cnt == 4)) flush(tnear, e64);
-  }
   // One term's classification, independent of every other term's (so the kernel interleaves it with the mma chain
-  // of the next step): adds a far term to `add` (the caller folds it into ffar) and says whether the term is near.
-  // gap = skip - tnear.
-  __device__ __forceinline__ bool classify(double L, float gap, float& add) const {
+  // of the next step): adds a far term to `add` (the caller folds it into ffar), counts it in `nfar` (lab counters)
+  // and says whether the term is near.  gap = skip - tnear.
+  __device__ __forceinline__ bool classify(double L, float gap, float& add, int& nfar) const {
     const float df = __double2float_rn(L - R);  // cold (R = -inf): +inf -> near; L = -inf or NaN: dropped
     const bool near = df > thn;
     const bool far = !near && df > thn - gap;
     const float e = ex2_approx(df * 1.44269504f);
     add += far ? e : 0.0f;
+    nfar += far ? 1 : 0;
     return near;
-  }
-  // park the near terms of one batch; one vote decides whether any lane has a near term at all.  Terms of the batch
-  // classified far against the old base stay far (exact enough by construction) even if a flush raises base.
-  template <int N>
-  __device__ __forceinline__ void park_batch(const double (&L)[N], const bool (&near)[N], float tnear,
-                                             const double* e64) {
-    bool any = false;
-#pragma unroll
-    for (int i = 0; i < N; ++i) any = any || near[i];
-    if (__any_sync(0xffffffffu, any)) {
-#pragma unroll
-      for (int i = 0; i < N; ++i)
-        if (__any_sync(0xffffffffu, near[i])) park(L[i], near[i], tnear, e64);
-    }
   }
   // the lane's (max, sum) pair for lse_merge, relative to base (s e^(R - base); R = base = -inf: (-inf, 0))
   __device__ __forceinline__ double2 result(const double* e64) const {
@@ -1628,6 +1635,32 @@ __device__ __forceinline__ void dmma_16x8x8(double& d0, double& d1, double& d2, 
                : "+d"(d0), "+d"(d1), "+d"(d2), "+d"(d3)
                : "d"(a0), "d"(a1), "d"(a2), "d"(a3), "d"(b0), "d"(b1));
 }
+// Dynamic shared memory of one k_logpdf_mma CTA: the TMA stages (table tiles, constants, full / empty barriers),
+// then the near-term ring.  The ring takes D slots per (warp, candidate group, lane), 8 B each, laid out
+// [slot][warp][group][lane].  D is as deep as the memory the stages leave allows at the CTAs per SM they allow (at
+// most MINB; 228 KB per SM, 1 KB reserved and the 512 B uni_exp table per CTA), capped at max(8, 2 NVG), and must
+// hold at least the NVG values one step can park: a warp flushes once a lane has more than D - NVG terms parked.
+template <int PB, int M, int KG, int NT, int TK, int ST, int MINB>
+struct MmaSmem {
+  static constexpr size_t stages = (size_t)ST * TK * PB * 8 + (size_t)ST * TK * 8 + (size_t)ST * 16;
+  static constexpr int NVG = 2 * KG;                                // values per lane, candidate group and step
+  static constexpr int RS = (NT / 32) * M * 32;                     // doubles between two slots of a lane's ring
+  static constexpr size_t kSm = 228 * 1024, kCta = 1024 + 64 * 8;
+  static constexpr size_t ctas_ = kSm / (stages + kCta);
+  static constexpr size_t ctas = ctas_ < (size_t)MINB ? ctas_ : (size_t)MINB;
+  static constexpr size_t fit = (kSm / ctas - kCta - stages) / (RS * 8);
+  static constexpr int cap = (2 * NVG > 8) ? 2 * NVG : 8;
+  static constexpr int D = (fit < (size_t)cap) ? (int)fit : cap;
+  static_assert(D >= NVG, "the near-term ring does not fit beside the TMA stages: fewer stages or a shorter tile");
+  static constexpr size_t bytes = stages + (size_t)D * RS * 8;
+};
+
+#ifdef TPE_LAB
+// lab counters of k_logpdf_mma<..., DBG = 5> (summed over launches until read by tpe_lab_mma_counters): near terms,
+// far terms, flushes by the vote (per warp and candidate group), terms parked at those flushes, ring slots they walked
+__device__ unsigned long long g_mma_lab_count[5];
+#endif
+
 // KG kernel groups (8 kernels each) per step of a warp: KG * M independent m8n8k4 chains (M = 1), or KG * M / 2
 // m16n8k8 chains (M even, two candidate groups per instruction).  The steps are software-pipelined: a warp issues
 // the chains of step s + 1 before it classifies the sums of step s, so the DMMA latency of one step hides behind
@@ -1647,6 +1680,8 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
   double* csts = tiles + (size_t)ST * TK * PB;                                     // ST * TK
   uint64_t* full = reinterpret_cast<uint64_t*>(csts + (size_t)ST * TK);            // ST
   uint64_t* empty = full + ST;                                                     // ST
+  using SM = MmaSmem<PB, M, KG, NT, TK, ST, MINB>;
+  double* ring = reinterpret_cast<double*>(empty + ST) + (threadIdx.x >> 5) * M * 32 + (threadIdx.x & 31);
   const int tid = threadIdx.x;
   const int lane = tid & 31;
   const int g = lane >> 2, q = lane & 3;
@@ -1762,9 +1797,15 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
   };
 
   LseRef acc[M];
+  unsigned long long gpend[M];   // gmax slot as read for the next exchange of maxima
 #pragma unroll
-  for (int m = 0; m < M; ++m) acc[m].init();
+  for (int m = 0; m < M; ++m) {
+    acc[m].init((unsigned)__cvta_generic_to_shared(ring + m * 32));
+    gpend[m] = ld_relaxed_gpu(gmax + wbase + 8 * m + g);
+  }
   const float lim_near = (float)lse_near, lim_gap = (float)(lse_skip - lse_near);
+  int lab_far = 0;                                   // lab counters (DBG = 5)
+  unsigned lab_near = 0, lab_flush = 0, lab_occ = 0, lab_walk = 0;
 
   constexpr int NV = 2 * KG * M;   // sums per lane and step: value j = (m, u, h) = (j / 2KG, j % 2KG / 2, j % 2)
   double cur[KG][M][2], nxt[KG][M][2];
@@ -1782,7 +1823,7 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
 #pragma unroll
         for (int m = 0; m < M; ++m) {
           acc[m].roll();
-          acc[m].sync_global(gmax + wbase + 8 * m + g, lim_near, s_e64);
+          acc[m].sync_global(gmax + wbase + 8 * m + g, gpend[m], lim_near, s_e64);
         }
       } else if ((kc & 15) == 0) {  // long tiles (small PB): keep the fp32 runs at <= 32 terms
 #pragma unroll
@@ -1797,7 +1838,7 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
     auto cls = [&](int j) {
       const int m = j / (2 * KG), u = (j % (2 * KG)) / 2, h = j & 1;
       if constexpr (DBG == 1 || DBG == 4) acc[m].s += cur[u][m][h];
-      else nr[m][j % (2 * KG)] = acc[m].classify(cur[u][m][h], lim_gap, add[m]);
+      else nr[m][j % (2 * KG)] = acc[m].classify(cur[u][m][h], lim_gap, add[m], lab_far);
     };
     // level i of the next chain is followed by the values j with j * NL / NV == i
     auto work = [&](int i) {
@@ -1829,14 +1870,24 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
 #pragma unroll
       for (int m = 0; m < M; ++m) {
         acc[m].ffar += add[m];
-        if constexpr (DBG == 0) {
-          double vals[2 * KG];
+        if constexpr (DBG == 0 || DBG == 5) {
+          // terms classified far against the old base stay far (exact enough by construction) even if the flush
+          // raises base
 #pragma unroll
-          for (int u = 0; u < KG; ++u) {
-            vals[2 * u] = cur[u][m][0];
-            vals[2 * u + 1] = cur[u][m][1];
+          for (int i = 0; i < 2 * KG; ++i) {
+            acc[m].template park<SM::RS>(cur[i / 2][m][i % 2], nr[m][i]);
+            if constexpr (DBG == 5) lab_near += nr[m][i] ? 1 : 0;
           }
-          acc[m].template park_batch<2 * KG>(vals, nr[m], lim_near, s_e64);
+          const unsigned slot0 = (unsigned)__cvta_generic_to_shared(ring + m * 32);
+          if (__any_sync(0xffffffffu, acc[m].wp > slot0 + (SM::D - SM::NVG) * SM::RS * 8)) {
+            if constexpr (DBG == 5) {
+              const int cnt = acc[m].template parked<SM::RS>(slot0);
+              lab_flush += 1;
+              lab_occ += cnt;
+              lab_walk += __reduce_max_sync(0xffffffffu, cnt);
+            }
+            acc[m].template flush<SM::RS>(ring + m * 32, lim_near, s_e64);
+          }
         }
       }
     }
@@ -1853,7 +1904,7 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
   }
 #pragma unroll
   for (int m = 0; m < M; ++m) {
-    acc[m].flush(lim_near, s_e64);
+    acc[m].template flush<SM::RS>(ring + m * 32, lim_near, s_e64);
     acc[m].roll();
     const double2 r = acc[m].result(s_e64);
     double mm = r.x, ss = r.y;
@@ -1864,6 +1915,20 @@ k_logpdf_mma(const double* __restrict__ tabm, const double* __restrict__ ckk, in
     }
     if (q == 0) part[blockIdx.y * ct_stride + wbase + 8 * m + g] = make_double2(mm + ha[m], ss);
   }
+#ifdef TPE_LAB
+  if constexpr (DBG == 5) {
+    const unsigned nn = __reduce_add_sync(0xffffffffu, lab_near);
+    const unsigned nf = __reduce_add_sync(0xffffffffu, (unsigned)lab_far);
+    const unsigned no = __reduce_add_sync(0xffffffffu, lab_occ);
+    if (lane == 0) {
+      atomicAdd(&g_mma_lab_count[0], (unsigned long long)nn);
+      atomicAdd(&g_mma_lab_count[1], (unsigned long long)nf);
+      atomicAdd(&g_mma_lab_count[2], (unsigned long long)lab_flush);
+      atomicAdd(&g_mma_lab_count[3], (unsigned long long)no);
+      atomicAdd(&g_mma_lab_count[4], (unsigned long long)lab_walk);
+    }
+  }
+#endif
 }
 
 // ================================================================================================
