@@ -38,14 +38,16 @@ extern "C" {
 /* 7: + tpe_hypervolume_history */
 /* 8: + tpe_pareto_front */
 /* 9: + tpe_fanova_variances */
-#define TPE_ABI_VERSION 9
+/* 10: + tpe_gp_set_data, tpe_gp_loss, tpe_gp_posterior, TPE_E_NOTPD */
+#define TPE_ABI_VERSION 10
 
 enum {
   TPE_OK = 0,
   TPE_E_INVALID = -1,  /* bad argument (mirrors the reference's ValueError) */
   TPE_E_CUDA = -2,     /* CUDA runtime failure */
   TPE_E_STATE = -3,    /* call order violated (e.g. suggest before history/space are set) */
-  TPE_E_NOMEM = -4
+  TPE_E_NOMEM = -4,
+  TPE_E_NOTPD = -5     /* a Gaussian-process covariance is not positive definite (torch's Cholesky LinAlgError) */
 };
 
 /* optuna/distributions.py: FloatDistribution :109, IntDistribution :310, CategoricalDistribution :470 */
@@ -292,6 +294,24 @@ int tpe_fanova_variances(tpe_ctx* ctx, int32_t n_trees, const int64_t* node_offs
                          const int32_t* right, const int32_t* feature, const double* threshold, const double* value,
                          int32_t n_features, const double* bounds, int32_t n_params, const int32_t* param_offsets,
                          const int32_t* raw_features, double* tree_variance, double* marginal_variance);
+/* Gaussian process of the terminator's regret bound (RegretBoundEvaluator, optuna/terminator/improvement/
+ * evaluator.py:142-177), fp64.  Kept apart from the history and the suggestion state.
+ * tpe_gp_set_data replaces the GPRegressor's training data (optuna/_gp/gp.py:94-118): X [n, P] normalised
+ * parameters, y [n] standardised values, is_categorical [P] (0 / 1); n >= 1, P >= 1, all finite.  Allocates two
+ * n x n matrices; TPE_E_INVALID naming the need when the device lacks the memory.
+ * tpe_gp_loss replaces loss_func of GPRegressor._fit_kernel_params without its prior term (gp.py:312-327,
+ * marginal_log_likelihood :252-285 and its backward): raw [P + 2] = log inverse squared lengthscales, log kernel
+ * scale, log(noise_var - minimum_noise).  *loss = -log p(y), grad [P + 2] its gradient in raw.
+ * tpe_gp_posterior replaces _cache_matrix / posterior (gp.py:124-149, 215-250) and UCB / LCB (optuna/_gp/acqf.py:
+ * 185-214): params [P + 2] = inverse squared lengthscales, kernel scale, noise_var; Xq [m, P]; ucb, lcb [m] =
+ * mean +- sqrt(beta var), var clamped at 0.
+ * Both return TPE_E_NOTPD when a Cholesky pivot is <= 0 or NaN; tpe_gp_loss also when a raw parameter is NaN or
+ * large enough that a kernel parameter is not finite (the reference's Cholesky fails there too). */
+int tpe_gp_set_data(tpe_ctx* ctx, const double* X, const double* y, const uint8_t* is_categorical, int64_t n,
+                    int32_t P);
+int tpe_gp_loss(tpe_ctx* ctx, const double* raw, double minimum_noise, double* loss, double* grad);
+int tpe_gp_posterior(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta, double* ucb,
+                     double* lcb);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

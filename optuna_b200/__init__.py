@@ -7,7 +7,8 @@ sm_90a CUDA through a C ABI (include/optuna_b200_tpe.h) bound with ctypes.
 from .engine import ParamSpec, TPEEngine  # noqa: F401
 
 __all__ = ["ParamSpec", "TPEEngine", "B200TPESampler", "hypervolume_history", "plot_hypervolume_history",
-           "best_trials", "pareto_front_info", "plot_pareto_front", "FanovaImportanceEvaluator"]
+           "best_trials", "pareto_front_info", "plot_pareto_front", "FanovaImportanceEvaluator",
+           "RegretBoundEvaluator"]
 
 
 def __getattr__(name):
@@ -21,4 +22,7 @@ def __getattr__(name):
     if name == "FanovaImportanceEvaluator":
         from .importance import FanovaImportanceEvaluator
         return FanovaImportanceEvaluator
+    if name == "RegretBoundEvaluator":
+        from .terminator import RegretBoundEvaluator
+        return RegretBoundEvaluator
     raise AttributeError(name)

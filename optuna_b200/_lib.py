@@ -12,7 +12,7 @@ _HERE = os.path.dirname(os.path.abspath(__file__))
 # TPE_LAB=1 loads the lab build (experimental kernels selectable by TPE_MMA_LAB etc., see DESIGN.md section 6)
 LIB_PATH = os.path.join(_HERE, "libtpe_b200_lab.so" if os.environ.get("TPE_LAB") == "1" else "libtpe_b200.so")
 
-TPE_OK, TPE_E_INVALID, TPE_E_CUDA, TPE_E_STATE, TPE_E_NOMEM = 0, -1, -2, -3, -4
+TPE_OK, TPE_E_INVALID, TPE_E_CUDA, TPE_E_STATE, TPE_E_NOMEM, TPE_E_NOTPD = 0, -1, -2, -3, -4, -5
 KIND_FLOAT, KIND_INT, KIND_CAT = 0, 1, 2
 CAT_COMPLETE, CAT_PRUNED, CAT_INFEASIBLE, CAT_RUNNING, CAT_EXCLUDED = 0, 1, 2, 3, 4
 
@@ -74,6 +74,9 @@ SYMBOLS = {
     "tpe_pareto_front": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P]),
     "tpe_fanova_variances": (C.c_int, [_P, C.c_int32, _P, _P, _P, _P, _P, _P, C.c_int32, _P, C.c_int32, _P, _P,
                                        _P, _P]),
+    "tpe_gp_set_data": (C.c_int, [_P, _P, _P, _P, C.c_int64, C.c_int32]),
+    "tpe_gp_loss": (C.c_int, [_P, _P, C.c_double, C.POINTER(C.c_double), _P]),
+    "tpe_gp_posterior": (C.c_int, [_P, _P, _P, C.c_int64, C.c_double, _P, _P]),
     "tpe_get_candidates": (C.c_int, [_P, _P, _P, _P]),
     "tpe_logpdf": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P]),
     "tpe_last_timing": (C.c_int, [_P, _P, _P]),
@@ -84,7 +87,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 9  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 10  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

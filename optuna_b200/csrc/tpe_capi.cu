@@ -22,6 +22,7 @@
 #include "tpe_hvhist.cuh"
 #include "tpe_pareto.cuh"
 #include "tpe_fanova.cuh"
+#include "tpe_gp.cuh"
 #include "tpe_uni.cuh"
 #include "tpe_mixed.cuh"
 #include "tpe_tcscreen.cuh"
@@ -109,6 +110,26 @@ struct Estimator {
     for (DevBuf* b : {&uord, &us32, &usmi, &usc, &umeta, &ucoef, &ubox, &ubstart, &utlist, &mxc, &mxd, &tcs_h, &tcs_ak, &tcs_ak64, &tabm, &hb, &ckk, &cls, &dtab, &offgrid, &tab32, &tab64p, &d32, &rows, &pos, &wstage, &wpart, &w, &logw, &cdf, &mu, &sigma, &cst_part, &cst, &tabp, &tabc, &colprm, &tab,
                       &part, &fix})
       b->release();
+  }
+};
+
+// Gaussian process of the terminator's regret bound (tpe_gp_*, tpe_gp.cuh): the data of tpe_gp_set_data and the
+// exact-size buffers -- two n x n matrices (A holds at least 1024 rows of n for the posterior's cross covariance)
+struct GpState {
+  int64_t n = 0;
+  int32_t P = 0;
+  double *X = nullptr, *y = nullptr, *A = nullptr, *B = nullptr, *W = nullptr, *u = nullptr, *alpha = nullptr;
+  double *prm = nullptr, *part = nullptr, *scal = nullptr, *grad = nullptr, *Xq = nullptr, *ucb = nullptr,
+         *lcb = nullptr;
+  uint8_t* cat = nullptr;
+  int* fail = nullptr;
+  int64_t part_cap = 0, xq_cap = 0;
+  bool ready = false;   // tpe_gp_set_data completed: every buffer above is allocated
+  void release() {
+    for (void* p : {(void*)X, (void*)y, (void*)A, (void*)B, (void*)W, (void*)u, (void*)alpha, (void*)prm, (void*)part,
+                    (void*)scal, (void*)grad, (void*)Xq, (void*)ucb, (void*)lcb, (void*)cat, (void*)fail})
+      if (p) cudaFree(p);
+    *this = GpState();
   }
 };
 
@@ -245,6 +266,7 @@ struct tpe_ctx {
   uint64_t uni_ord_lineage = 0;        // ... and what else it belongs to
   int32_t uni_ord_col = -1;
   int64_t uni_ord_K = -1;
+  GpState gp;
 };
 
 namespace {
@@ -2205,6 +2227,7 @@ void tpe_ctx_destroy(tpe_ctx* ctx) {
     b->release();
   ctx->est[0].release();
   ctx->est[1].release();
+  ctx->gp.release();
   if (ctx->res_host) cudaFreeHost(ctx->res_host);
   if (ctx->mt_host) cudaFreeHost(ctx->mt_host);
   if (ctx->up_host) cudaFreeHost(ctx->up_host);
@@ -3478,6 +3501,226 @@ int tpe_probe_fp64_tflops(tpe_ctx* ctx, double* tflops) {
   out.release();
   const double flops = 2.0 * 8.0 * (double)iters * blocks * threads;
   *tflops = flops / (best * 1e-3) / 1e12;
+  return TPE_OK;
+}
+
+// ---- Gaussian process of the terminator's regret bound (tpe_gp.cuh) ------------------------------------------------
+static constexpr int64_t kGpQmax = 1024;   // query rows per posterior chunk (cross covariance rows held in A)
+static constexpr int kGpGradBlocks = 1024; // CTAs of k_gp_grad at most: fixed, so the partial sums' order is too
+
+static int64_t gp_grad_blocks(int64_t n) {
+  const int64_t total = n * (n + 1) / 2;
+  return std::min<int64_t>((total + gp::GRAD_THREADS - 1) / gp::GRAD_THREADS, kGpGradBlocks);
+}
+
+static void gp_gemm(cudaStream_t st, const double* A, int64_t lda, const double* B, int64_t ldb, double* out,
+                    int64_t ldc, int64_t M, int64_t N, int64_t K, double alpha, int flags) {
+  if (M <= 0 || N <= 0) return;
+  const dim3 grid((unsigned)((N + gp::NB - 1) / gp::NB), (unsigned)((M + gp::NB - 1) / gp::NB));
+  gp::k_gp_gemm<<<grid, 128, 0, st>>>(A, lda, B, ldb, out, ldc, (int)M, (int)N, (int)K, alpha, flags);
+}
+
+// C at gp.prm into A, then L (right-looking blocked Cholesky) in A and L^-1 (blocked TRTRI) in B; gp.fail is set when
+// a pivot is <= 0 or NaN.  Then u = L^-1 y, [sum log L_ii, u.u] in gp.scal and alpha = L^-T u.
+static void gp_factor(tpe_ctx* ctx) {
+  GpState& g = ctx->gp;
+  cudaStream_t st = ctx->stream;
+  const int64_t n = g.n;
+  const int NB = gp::NB;
+  cudaMemsetAsync(g.fail, 0, sizeof(int), st);
+  const unsigned nt = (unsigned)((n + 31) / 32);
+  gp::k_gp_cov<<<dim3(nt, nt), dim3(32, 32), 0, st>>>(g.X, g.cat, g.prm, g.P, (int)n, g.A);
+  double *A = g.A, *B = g.B;
+  for (int64_t k0 = 0; k0 < n; k0 += NB) {
+    const int64_t nb = std::min<int64_t>(NB, n - k0), r0 = k0 + nb, m = n - r0;
+    gp::k_gp_potrf_diag<<<1, 256, 0, st>>>(A, B, (int)n, (int)k0, (int)nb, g.fail);
+    if (m > 0) {
+      // panel TRSM in place: L21 = A21 L11^-T, with L11^-1 from the diagonal block of B
+      gp_gemm(st, A + r0 * n + k0, n, B + k0 * n + k0, n, A + r0 * n + k0, n, m, nb, nb, 1.0, 0);
+      // trailing SYRK: A22 -= L21 L21^T over the lower triangle
+      gp_gemm(st, A + r0 * n + k0, n, A + r0 * n + k0, n, A + r0 * n + r0, n, m, m, nb, -1.0,
+              gp::GF_LOWER | gp::GF_ACCUM);
+    }
+  }
+  // TRTRI, last block column first: L^-1[r0:, k0:r0] = -(L^-1[r0:, r0:] L[r0:, k0:r0]) L^-1[k0:r0, k0:r0]
+  for (int64_t k0 = ((n - 1) / NB) * NB; k0 >= 0; k0 -= NB) {
+    const int64_t nb = std::min<int64_t>(NB, n - k0), r0 = k0 + nb, m = n - r0;
+    if (m == 0) continue;
+    gp_gemm(st, B + r0 * n + r0, n, A + r0 * n + k0, n, g.W, NB, m, nb, m, 1.0, gp::GF_TB | gp::GF_KHI_ROW);
+    gp_gemm(st, g.W, NB, B + k0 * n + k0, n, B + r0 * n + k0, n, m, nb, nb, -1.0, gp::GF_TB);
+  }
+  gp::k_gp_trmv_lower<<<(unsigned)((n + 7) / 8), 256, 0, st>>>(B, g.y, (int)n, g.u);
+  gp::k_gp_stats<<<1, 256, 0, st>>>(A, g.u, (int)n, g.scal);
+  gp::k_gp_trmv_lower_t<<<(unsigned)((n + 31) / 32), 256, 0, st>>>(B, g.u, (int)n, g.alpha);
+}
+
+// the allocations and uploads of tpe_gp_set_data; on failure the caller releases what was allocated
+static int gp_upload(tpe_ctx* ctx, const double* X, const double* y, const uint8_t* is_categorical, int64_t n,
+                     int32_t P, size_t a_elems, size_t b_elems, int64_t part) {
+  GpState& g = ctx->gp;
+  g.n = n;
+  g.P = P;
+  CU(cudaMalloc(&g.A, a_elems * 8));
+  CU(cudaMalloc(&g.B, b_elems * 8));
+  CU(cudaMalloc(&g.W, (size_t)n * gp::NB * 8));
+  CU(cudaMalloc(&g.X, (size_t)n * P * 8));
+  CU(cudaMalloc(&g.y, n * 8));
+  CU(cudaMalloc(&g.u, n * 8));
+  CU(cudaMalloc(&g.alpha, n * 8));
+  CU(cudaMalloc(&g.prm, (P + 2) * 8));
+  CU(cudaMalloc(&g.part, part * 8));
+  g.part_cap = part;
+  CU(cudaMalloc(&g.scal, 2 * 8));
+  CU(cudaMalloc(&g.grad, (P + 2) * 8));
+  CU(cudaMalloc(&g.cat, P));
+  CU(cudaMalloc(&g.fail, sizeof(int)));
+  std::vector<uint8_t> cat(P);
+  for (int d = 0; d < P; ++d) cat[d] = is_categorical[d] ? 1 : 0;
+  CU(cudaMemsetAsync(g.B, 0, b_elems * 8, ctx->stream));   // L^-1: the upper triangle stays zero
+  CU(cudaMemcpyAsync(g.X, X, (size_t)n * P * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(g.y, y, n * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaMemcpyAsync(g.cat, cat.data(), P, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  return TPE_OK;
+}
+
+// replaces GPRegressor(...) construction (optuna/_gp/gp.py:94-118): the training data of the fit
+int tpe_gp_set_data(tpe_ctx* ctx, const double* X, const double* y, const uint8_t* is_categorical, int64_t n,
+                    int32_t P) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (n < 1 || P < 1 || n > (int64_t)1 << 30) return fail(ctx, TPE_E_INVALID, "bad GP sizes (n %lld, P %d)", (long long)n, P);
+  if (!X || !y || !is_categorical) return fail(ctx, TPE_E_INVALID, "bad GP arguments");
+  for (int64_t i = 0; i < n * P; ++i)
+    if (!std::isfinite(X[i])) return fail(ctx, TPE_E_INVALID, "GP inputs hold a non-finite value");
+  for (int64_t i = 0; i < n; ++i)
+    if (!std::isfinite(y[i])) return fail(ctx, TPE_E_INVALID, "GP targets hold a non-finite value");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  GpState& g = ctx->gp;
+  g.release();
+  const int64_t npass = (P + gp::GRAD_DC - 1) / gp::GRAD_DC;
+  const int64_t part = std::max<int64_t>(npass * kGpGradBlocks * (gp::GRAD_DC + 2), kGpQmax * ((n + gp::NB - 1) / gp::NB));
+  const size_t a_elems = (size_t)std::max<int64_t>(n, kGpQmax) * n, b_elems = (size_t)n * n;
+  // A, B, the TRTRI panel, X / y / u / alpha, the partial sums and scalars, and the posterior's query buffers for
+  // the evaluator's n + 2048 points (Xq, ucb, lcb)
+  const size_t n_query = (size_t)n + 2048;
+  const size_t need = 8 * (a_elems + b_elems + (size_t)n * gp::NB + (size_t)n * (P + 3) + (size_t)part + 3 * (P + 2) +
+                           2 + n_query * (P + 2)) + P + sizeof(int);
+  size_t free_b = 0, total_b = 0;
+  CU(cudaMemGetInfo(&free_b, &total_b));
+  if (need > free_b)
+    return fail(ctx, TPE_E_INVALID,
+                "the Gaussian process over n = %lld points needs %.2f GB of device memory (two n x n fp64 matrices), "
+                "device %d has %.2f GB free",
+                (long long)n, need / 1e9, ctx->device, free_b / 1e9);
+  const int rc = gp_upload(ctx, X, y, is_categorical, n, P, a_elems, b_elems, part);
+  if (rc != TPE_OK) {
+    // a partial allocation (free memory can shrink after the check on a shared device) leaves no usable state
+    cudaStreamSynchronize(ctx->stream);
+    g.release();
+    return rc;
+  }
+  g.ready = true;
+  return TPE_OK;
+}
+
+// replaces loss_func of GPRegressor._fit_kernel_params without the prior (optuna/_gp/gp.py:312-327, with
+// marginal_log_likelihood :252-285 and its autograd backward): -log p(y | raw) and its gradient in raw
+int tpe_gp_loss(tpe_ctx* ctx, const double* raw, double minimum_noise, double* loss, double* grad) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  GpState& g = ctx->gp;
+  if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
+  if (!raw || !loss || !grad) return fail(ctx, TPE_E_INVALID, "bad GP loss arguments");
+  const int P = g.P;
+  if (!std::isfinite(minimum_noise) || minimum_noise < 0.0) return fail(ctx, TPE_E_INVALID, "bad minimum noise");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  std::vector<double> prm(P + 2);
+  for (int d = 0; d < P; ++d) prm[d] = std::exp(raw[d]);
+  prm[P] = std::exp(raw[P]);
+  const double noise_excess = std::exp(raw[P + 1]);
+  prm[P + 1] = noise_excess + minimum_noise;
+  // a NaN or +inf raw parameter (a line-search iterate) makes the reference's covariance non-finite and its
+  // Cholesky fail: the same error here, so that the fit retries and falls back the same way
+  for (int d = 0; d < P + 2; ++d)
+    if (!std::isfinite(prm[d]))
+      return fail(ctx, TPE_E_NOTPD, "the GP covariance is not positive definite (non-finite kernel parameters)");
+  cudaStream_t st = ctx->stream;
+  CU(cudaMemcpyAsync(g.prm, prm.data(), (P + 2) * 8, cudaMemcpyHostToDevice, st));
+  gp_factor(ctx);
+  const int64_t n = g.n;
+  // C^-1 = L^-T L^-1 over the lower triangle, into A
+  gp_gemm(st, g.B, n, g.B, n, g.A, n, n, n, n, 1.0, gp::GF_TA | gp::GF_TB | gp::GF_LOWER | gp::GF_KLO_ROW);
+  const int64_t nblk = gp_grad_blocks(n);
+  for (int d0 = 0; d0 < P; d0 += gp::GRAD_DC) {
+    double* part = g.part + (int64_t)(d0 / gp::GRAD_DC) * nblk * (gp::GRAD_DC + 2);
+    gp::k_gp_grad<gp::GRAD_DC><<<(unsigned)nblk, gp::GRAD_THREADS, 0, st>>>(g.A, g.X, g.cat, g.prm, g.alpha, P,
+                                                                           (int)n, d0, part);
+    gp::k_gp_grad_finish<gp::GRAD_DC><<<1, 32, 0, st>>>(part, (int)nblk, g.prm, P, d0, g.grad);
+  }
+  gp::k_gp_grad_tail<<<1, 1, 0, st>>>(g.prm, noise_excess, P, g.grad);
+  CU(cudaGetLastError());
+  int failed = 0;
+  double scal[2];
+  CU(cudaMemcpyAsync(&failed, g.fail, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(scal, g.scal, 2 * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(grad, g.grad, (P + 2) * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (failed) return fail(ctx, TPE_E_NOTPD, "the GP covariance is not positive definite (Cholesky pivot <= 0 or NaN)");
+  // marginal_log_likelihood's order: (logdet_part + const) + quad_part, negated
+  const double mll = (-scal[0] + -0.5 * (double)n * std::log(2.0 * M_PI)) + -0.5 * scal[1];
+  *loss = -mll;
+  return TPE_OK;
+}
+
+// replaces GPRegressor._cache_matrix + posterior (optuna/_gp/gp.py:124-149, 215-250) and UCB / LCB.eval_acqf
+// (optuna/_gp/acqf.py:185-214): mean +- sqrt(beta var) at m query points, for params = [l_1 .. l_P, ks, noise_var]
+int tpe_gp_posterior(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta, double* ucb,
+                     double* lcb) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  GpState& g = ctx->gp;
+  if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
+  if (!params || !Xq || !ucb || !lcb || m < 1) return fail(ctx, TPE_E_INVALID, "bad GP posterior arguments");
+  const int P = g.P;
+  for (int d = 0; d < P + 2; ++d)
+    if (!std::isfinite(params[d])) return fail(ctx, TPE_E_INVALID, "kernel parameters hold a non-finite value");
+  if (!std::isfinite(beta) || beta < 0.0) return fail(ctx, TPE_E_INVALID, "bad beta");
+  for (int64_t i = 0; i < m * P; ++i)
+    if (!std::isfinite(Xq[i])) return fail(ctx, TPE_E_INVALID, "query points hold a non-finite value");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  cudaStream_t st = ctx->stream;
+  if (m > g.xq_cap) {
+    for (double** p : {&g.Xq, &g.ucb, &g.lcb}) {
+      if (*p) cudaFree(*p);
+      *p = nullptr;
+    }
+    g.xq_cap = 0;
+    CU(cudaMalloc(&g.Xq, (size_t)m * P * 8));
+    CU(cudaMalloc(&g.ucb, m * 8));
+    CU(cudaMalloc(&g.lcb, m * 8));
+    g.xq_cap = m;
+  }
+  CU(cudaMemcpyAsync(g.prm, params, (P + 2) * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(g.Xq, Xq, (size_t)m * P * 8, cudaMemcpyHostToDevice, st));
+  gp_factor(ctx);
+  const int64_t n = g.n, ntiles = (n + gp::NB - 1) / gp::NB;
+  for (int64_t q0 = 0; q0 < m; q0 += kGpQmax) {
+    const int64_t Q = std::min(kGpQmax, m - q0);
+    gp::k_gp_cross<<<dim3((unsigned)((n + 127) / 128), (unsigned)Q), 128, 0, st>>>(g.Xq + q0 * P, g.X, g.cat, g.prm,
+                                                                                  P, (int)n, (int)Q, g.A);
+    // squared norms of L^-1 k*, per query and column tile
+    gp_gemm(st, g.A, n, g.B, n, g.part, 0, Q, n, n, 1.0, gp::GF_KHI_COL | gp::GF_SQSUM);
+    gp::k_gp_post_finish<<<(unsigned)((Q + 7) / 8), 256, 0, st>>>(g.A, g.alpha, g.part, (int)ntiles, g.prm, P, (int)n,
+                                                                  (int)Q, beta, g.ucb + q0, g.lcb + q0);
+  }
+  CU(cudaGetLastError());
+  int failed = 0;
+  CU(cudaMemcpyAsync(&failed, g.fail, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(ucb, g.ucb, m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(lcb, g.lcb, m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (failed) return fail(ctx, TPE_E_NOTPD, "the GP covariance is not positive definite (Cholesky pivot <= 0 or NaN)");
   return TPE_OK;
 }
 

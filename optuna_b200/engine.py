@@ -39,6 +39,12 @@ def _f64(a, shape=None) -> np.ndarray:
     return out
 
 
+class GPCholeskyError(RuntimeError):
+    """The Gaussian-process covariance is not positive definite: a Cholesky pivot was <= 0 or NaN.  A
+    ``RuntimeError``, like the ``LinAlgError`` torch's Cholesky raises, so that optuna's fit retries and falls back
+    the same way."""
+
+
 class TPEEngine:
     def __init__(self, device: int = 0) -> None:
         self._lib = _lib.load()
@@ -54,6 +60,7 @@ class TPEEngine:
         self._ncat = self._nnum = 0
         self._specs: list[ParamSpec] = []
         self._cols: list[int] = []
+        self._gp_P = 0
 
     # -- lifecycle -----------------------------------------------------------------------------
     def close(self) -> None:
@@ -76,6 +83,8 @@ class TPEEngine:
         msg = self._lib.tpe_last_error(self._h).decode()
         if rc == _lib.TPE_E_INVALID:
             raise ValueError(msg)
+        if rc == _lib.TPE_E_NOTPD:
+            raise GPCholeskyError(msg)
         raise RuntimeError(f"libtpe_b200 error {rc}: {msg}")
 
     # -- space / history -------------------------------------------------------------------------
@@ -416,6 +425,44 @@ class TPEEngine:
                                                    _ptr(val), bnd.shape[0], _ptr(bnd), n_params, _ptr(po),
                                                    _ptr(cols), _ptr(tree_var), _ptr(marg)))
         return tree_var, marg
+
+    def gp_set_data(self, X, y, is_categorical) -> None:
+        """Training data of the terminator's Gaussian process (tpe_gp_set_data): ``X`` [n, P] normalised parameters,
+        ``y`` [n] standardised values, ``is_categorical`` [P].  Allocates two n x n fp64 matrices on the device;
+        ``ValueError`` naming the need when it lacks the memory.  Leaves the history and the suggestion state of
+        this engine unchanged."""
+        Xa, ya = _f64(X), _f64(y)
+        cat = np.ascontiguousarray(is_categorical, dtype=np.uint8)
+        if Xa.ndim != 2 or ya.shape != (Xa.shape[0],) or cat.shape != (Xa.shape[1],):
+            raise ValueError(f"GP data must be X [n, P], y [n], is_categorical [P]; got {Xa.shape}, {ya.shape}, "
+                             f"{cat.shape}")
+        self._gp_P = 0   # a failed call leaves no GP data in the context either
+        self._check(self._lib.tpe_gp_set_data(self._h, _ptr(Xa), _ptr(ya), _ptr(cat), Xa.shape[0], Xa.shape[1]))
+        self._gp_P = Xa.shape[1]
+
+    def gp_loss(self, raw_params, minimum_noise: float) -> tuple[float, np.ndarray]:
+        """Negative marginal log-likelihood of the GP data and its gradient in the raw kernel parameters (log
+        inverse squared lengthscales, log kernel scale, log(noise_var - minimum_noise)) (tpe_gp_loss).  Raises
+        ``GPCholeskyError`` when the covariance is not positive definite."""
+        raw = _f64(raw_params)
+        if self._gp_P and raw.shape != (self._gp_P + 2,):   # without GP data the library reports that first
+            raise ValueError(f"raw_params must have {self._gp_P + 2} entries, got shape {raw.shape}")
+        loss = C.c_double()
+        grad = np.empty(raw.size)
+        self._check(self._lib.tpe_gp_loss(self._h, _ptr(raw), float(minimum_noise), C.byref(loss), _ptr(grad)))
+        return loss.value, grad
+
+    def gp_posterior(self, params, Xq, beta: float) -> tuple[np.ndarray, np.ndarray]:
+        """``(mean + sqrt(beta var), mean - sqrt(beta var))`` of the GP posterior at the rows of ``Xq`` [m, P], for
+        ``params`` = (inverse squared lengthscales, kernel scale, noise_var) (tpe_gp_posterior).  Raises
+        ``GPCholeskyError`` when the covariance is not positive definite."""
+        prm, xq = _f64(params), _f64(Xq)
+        if xq.ndim != 2 or (self._gp_P and (prm.shape != (self._gp_P + 2,) or xq.shape[1] != self._gp_P)):
+            raise ValueError(f"params must have {self._gp_P + 2} entries and Xq {self._gp_P} columns")
+        ucb, lcb = np.empty(xq.shape[0]), np.empty(xq.shape[0])
+        self._check(self._lib.tpe_gp_posterior(self._h, _ptr(prm), _ptr(xq), xq.shape[0], float(beta), _ptr(ucb),
+                                               _ptr(lcb)))
+        return ucb, lcb
 
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:
