@@ -39,7 +39,8 @@ extern "C" {
 /* 8: + tpe_pareto_front */
 /* 9: + tpe_fanova_variances */
 /* 10: + tpe_gp_set_data, tpe_gp_loss, tpe_gp_posterior, TPE_E_NOTPD */
-#define TPE_ABI_VERSION 10
+/* 11: + tpe_gp_loss_fixed_noise, tpe_gp_posterior_moments */
+#define TPE_ABI_VERSION 11
 
 enum {
   TPE_OK = 0,
@@ -294,8 +295,9 @@ int tpe_fanova_variances(tpe_ctx* ctx, int32_t n_trees, const int64_t* node_offs
                          const int32_t* right, const int32_t* feature, const double* threshold, const double* value,
                          int32_t n_features, const double* bounds, int32_t n_params, const int32_t* param_offsets,
                          const int32_t* raw_features, double* tree_variance, double* marginal_variance);
-/* Gaussian process of the terminator's regret bound (RegretBoundEvaluator, optuna/terminator/improvement/
- * evaluator.py:142-177), fp64.  Kept apart from the history and the suggestion state.
+/* Gaussian process of the terminator's improvement evaluators (RegretBoundEvaluator, optuna/terminator/improvement/
+ * evaluator.py:142-177, and EMMREvaluator, emmr.py:123-237), fp64.  Kept apart from the history and the suggestion
+ * state.
  * tpe_gp_set_data replaces the GPRegressor's training data (optuna/_gp/gp.py:94-118): X [n, P] normalised
  * parameters, y [n] standardised values, is_categorical [P] (0 / 1); n >= 1, P >= 1, all finite.  Allocates two
  * n x n matrices; TPE_E_INVALID naming the need when the device lacks the memory.
@@ -305,13 +307,22 @@ int tpe_fanova_variances(tpe_ctx* ctx, int32_t n_trees, const int64_t* node_offs
  * tpe_gp_posterior replaces _cache_matrix / posterior (gp.py:124-149, 215-250) and UCB / LCB (optuna/_gp/acqf.py:
  * 185-214): params [P + 2] = inverse squared lengthscales, kernel scale, noise_var; Xq [m, P]; ucb, lcb [m] =
  * mean +- sqrt(beta var), var clamped at 0.
- * Both return TPE_E_NOTPD when a Cholesky pivot is <= 0 or NaN; tpe_gp_loss also when a raw parameter is NaN or
- * large enough that a kernel parameter is not finite (the reference's Cholesky fails there too). */
+ * tpe_gp_loss_fixed_noise is tpe_gp_loss with deterministic_objective=True (gp.py:312-327): the noise is fixed at
+ * noise_var, raw[P + 1] is ignored and grad[P + 1] = 0.
+ * tpe_gp_posterior_moments replaces GPRegressor.posterior (gp.py:215-250) at m points: mean [m], var [m] clamped at
+ * 0; with n_joint in [2, 64] (and <= m) also the joint covariance of the first n_joint points, cov [n_joint *
+ * n_joint] row-major, diagonal clamped at 0 (joint=True); n_joint = 0 and cov = NULL for none.  One factorisation
+ * per call.
+ * All return TPE_E_NOTPD when a Cholesky pivot is <= 0 or NaN; the loss calls also when a raw parameter they read is
+ * NaN or large enough that a kernel parameter is not finite (the reference's Cholesky fails there too). */
 int tpe_gp_set_data(tpe_ctx* ctx, const double* X, const double* y, const uint8_t* is_categorical, int64_t n,
                     int32_t P);
 int tpe_gp_loss(tpe_ctx* ctx, const double* raw, double minimum_noise, double* loss, double* grad);
 int tpe_gp_posterior(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta, double* ucb,
                      double* lcb);
+int tpe_gp_loss_fixed_noise(tpe_ctx* ctx, const double* raw, double noise_var, double* loss, double* grad);
+int tpe_gp_posterior_moments(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, int32_t n_joint,
+                             double* mean, double* var, double* cov);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

@@ -8,7 +8,7 @@ from .engine import ParamSpec, TPEEngine  # noqa: F401
 
 __all__ = ["ParamSpec", "TPEEngine", "B200TPESampler", "hypervolume_history", "plot_hypervolume_history",
            "best_trials", "pareto_front_info", "plot_pareto_front", "FanovaImportanceEvaluator",
-           "RegretBoundEvaluator"]
+           "RegretBoundEvaluator", "EMMREvaluator"]
 
 
 def __getattr__(name):
@@ -22,7 +22,7 @@ def __getattr__(name):
     if name == "FanovaImportanceEvaluator":
         from .importance import FanovaImportanceEvaluator
         return FanovaImportanceEvaluator
-    if name == "RegretBoundEvaluator":
-        from .terminator import RegretBoundEvaluator
-        return RegretBoundEvaluator
+    if name in ("RegretBoundEvaluator", "EMMREvaluator"):
+        from . import terminator
+        return getattr(terminator, name)
     raise AttributeError(name)

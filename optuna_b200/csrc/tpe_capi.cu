@@ -3624,22 +3624,18 @@ int tpe_gp_set_data(tpe_ctx* ctx, const double* X, const double* y, const uint8_
   return TPE_OK;
 }
 
-// replaces loss_func of GPRegressor._fit_kernel_params without the prior (optuna/_gp/gp.py:312-327, with
-// marginal_log_likelihood :252-285 and its autograd backward): -log p(y | raw) and its gradient in raw
-int tpe_gp_loss(tpe_ctx* ctx, const double* raw, double minimum_noise, double* loss, double* grad) {
-  if (!ctx) return TPE_E_INVALID;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+// The body of tpe_gp_loss and tpe_gp_loss_fixed_noise, called under the context lock with the arguments checked:
+// l_d = exp(raw_d), ks = exp(raw_P), noise_var = noise_excess + noise_base.  The gradient in raw_{P+1} is
+// 1/2 noise_excess sum_i W_ii, so noise_excess = 0 (the noise held fixed) makes it 0.
+static int gp_loss_run(tpe_ctx* ctx, const double* raw, double noise_excess, double noise_base, double* loss,
+                       double* grad) {
   GpState& g = ctx->gp;
-  if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
-  if (!raw || !loss || !grad) return fail(ctx, TPE_E_INVALID, "bad GP loss arguments");
   const int P = g.P;
-  if (!std::isfinite(minimum_noise) || minimum_noise < 0.0) return fail(ctx, TPE_E_INVALID, "bad minimum noise");
   if (set_device(ctx)) return TPE_E_CUDA;
   std::vector<double> prm(P + 2);
   for (int d = 0; d < P; ++d) prm[d] = std::exp(raw[d]);
   prm[P] = std::exp(raw[P]);
-  const double noise_excess = std::exp(raw[P + 1]);
-  prm[P + 1] = noise_excess + minimum_noise;
+  prm[P + 1] = noise_excess + noise_base;
   // a NaN or +inf raw parameter (a line-search iterate) makes the reference's covariance non-finite and its
   // Cholesky fail: the same error here, so that the fit retries and falls back the same way
   for (int d = 0; d < P + 2; ++d)
@@ -3673,21 +3669,36 @@ int tpe_gp_loss(tpe_ctx* ctx, const double* raw, double minimum_noise, double* l
   return TPE_OK;
 }
 
-// replaces GPRegressor._cache_matrix + posterior (optuna/_gp/gp.py:124-149, 215-250) and UCB / LCB.eval_acqf
-// (optuna/_gp/acqf.py:185-214): mean +- sqrt(beta var) at m query points, for params = [l_1 .. l_P, ks, noise_var]
-int tpe_gp_posterior(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta, double* ucb,
-                     double* lcb) {
+// replaces loss_func of GPRegressor._fit_kernel_params without the prior (optuna/_gp/gp.py:312-327, with
+// marginal_log_likelihood :252-285 and its autograd backward): -log p(y | raw) and its gradient in raw
+int tpe_gp_loss(tpe_ctx* ctx, const double* raw, double minimum_noise, double* loss, double* grad) {
   if (!ctx) return TPE_E_INVALID;
   std::lock_guard<std::mutex> lk(ctx->mu);
+  if (!ctx->gp.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
+  if (!raw || !loss || !grad) return fail(ctx, TPE_E_INVALID, "bad GP loss arguments");
+  if (!std::isfinite(minimum_noise) || minimum_noise < 0.0) return fail(ctx, TPE_E_INVALID, "bad minimum noise");
+  return gp_loss_run(ctx, raw, std::exp(raw[ctx->gp.P + 1]), minimum_noise, loss, grad);
+}
+
+// the same with deterministic_objective=True (gp.py:317-321): the noise is noise_var, raw[P + 1] is not read and
+// grad[P + 1] = 0
+int tpe_gp_loss_fixed_noise(tpe_ctx* ctx, const double* raw, double noise_var, double* loss, double* grad) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  if (!ctx->gp.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
+  if (!raw || !loss || !grad) return fail(ctx, TPE_E_INVALID, "bad GP loss arguments");
+  if (!std::isfinite(noise_var) || noise_var < 0.0) return fail(ctx, TPE_E_INVALID, "bad noise variance");
+  return gp_loss_run(ctx, raw, 0.0, noise_var, loss, grad);
+}
+
+// The body of tpe_gp_posterior and tpe_gp_posterior_moments, called under the context lock with the arguments
+// checked: factorise at params, then per chunk of query rows the cross covariance, the squared norms of L^-1 k* and
+// k_gp_post_finish (moments: mean / var, else mean +- sqrt(beta var)).  With J > 0 also the joint covariance of the
+// first J query rows into cov [J * J].
+static int gp_posterior_run(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta,
+                            bool moments, int J, double* out0, double* out1, double* cov) {
   GpState& g = ctx->gp;
-  if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
-  if (!params || !Xq || !ucb || !lcb || m < 1) return fail(ctx, TPE_E_INVALID, "bad GP posterior arguments");
   const int P = g.P;
-  for (int d = 0; d < P + 2; ++d)
-    if (!std::isfinite(params[d])) return fail(ctx, TPE_E_INVALID, "kernel parameters hold a non-finite value");
-  if (!std::isfinite(beta) || beta < 0.0) return fail(ctx, TPE_E_INVALID, "bad beta");
-  for (int64_t i = 0; i < m * P; ++i)
-    if (!std::isfinite(Xq[i])) return fail(ctx, TPE_E_INVALID, "query points hold a non-finite value");
   if (set_device(ctx)) return TPE_E_CUDA;
   cudaStream_t st = ctx->stream;
   if (m > g.xq_cap) {
@@ -3712,16 +3723,63 @@ int tpe_gp_posterior(tpe_ctx* ctx, const double* params, const double* Xq, int64
     // squared norms of L^-1 k*, per query and column tile
     gp_gemm(st, g.A, n, g.B, n, g.part, 0, Q, n, n, 1.0, gp::GF_KHI_COL | gp::GF_SQSUM);
     gp::k_gp_post_finish<<<(unsigned)((Q + 7) / 8), 256, 0, st>>>(g.A, g.alpha, g.part, (int)ntiles, g.prm, P, (int)n,
-                                                                  (int)Q, beta, g.ucb + q0, g.lcb + q0);
+                                                                  (int)Q, beta, moments, g.ucb + q0, g.lcb + q0);
+    if (q0 == 0 && J > 0) {
+      // V = K L^-T for the first J rows (J <= min(m, 64), so all in this chunk) into the n x 64 TRTRI panel
+      // buffer, free after gp_factor
+      gp_gemm(st, g.A, n, g.B, n, g.W, n, J, n, n, 1.0, gp::GF_KHI_COL);
+    }
   }
+  if (J > 0)   // after the last chunk's k_gp_post_finish has read g.part (>= 18 432 entries, see tpe_gp_set_data)
+    gp::k_gp_joint_cov<<<(unsigned)((J * J + 7) / 8), 256, 0, st>>>(g.Xq, g.W, g.cat, g.prm, P, (int)n, J, g.part);
   CU(cudaGetLastError());
   int failed = 0;
   CU(cudaMemcpyAsync(&failed, g.fail, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(ucb, g.ucb, m * 8, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(lcb, g.lcb, m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out0, g.ucb, m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(out1, g.lcb, m * 8, cudaMemcpyDeviceToHost, st));
+  if (J > 0) CU(cudaMemcpyAsync(cov, g.part, (size_t)J * J * 8, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   if (failed) return fail(ctx, TPE_E_NOTPD, "the GP covariance is not positive definite (Cholesky pivot <= 0 or NaN)");
   return TPE_OK;
+}
+
+// the argument checks the two posterior entry points share
+static int gp_posterior_check(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, bool ok) {
+  GpState& g = ctx->gp;
+  if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
+  if (!params || !Xq || !ok || m < 1) return fail(ctx, TPE_E_INVALID, "bad GP posterior arguments");
+  for (int d = 0; d < g.P + 2; ++d)
+    if (!std::isfinite(params[d])) return fail(ctx, TPE_E_INVALID, "kernel parameters hold a non-finite value");
+  for (int64_t i = 0; i < m * g.P; ++i)
+    if (!std::isfinite(Xq[i])) return fail(ctx, TPE_E_INVALID, "query points hold a non-finite value");
+  return TPE_OK;
+}
+
+// replaces GPRegressor._cache_matrix + posterior (optuna/_gp/gp.py:124-149, 215-250) and UCB / LCB.eval_acqf
+// (optuna/_gp/acqf.py:185-214): mean +- sqrt(beta var) at m query points, for params = [l_1 .. l_P, ks, noise_var]
+int tpe_gp_posterior(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta, double* ucb,
+                     double* lcb) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  const int rc = gp_posterior_check(ctx, params, Xq, m, ucb && lcb);
+  if (rc != TPE_OK) return rc;
+  if (!std::isfinite(beta) || beta < 0.0) return fail(ctx, TPE_E_INVALID, "bad beta");
+  return gp_posterior_run(ctx, params, Xq, m, beta, false, 0, ucb, lcb, nullptr);
+}
+
+// replaces GPRegressor._cache_matrix + posterior (gp.py:124-149, 215-250): mean and var at m query points, and with
+// n_joint in [2, 64] the joint covariance of the first n_joint of them (joint=True)
+int tpe_gp_posterior_moments(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, int32_t n_joint,
+                             double* mean, double* var, double* cov) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  const int rc = gp_posterior_check(ctx, params, Xq, m, mean && var);
+  if (rc != TPE_OK) return rc;
+  const bool joint_ok = n_joint == 0 ? cov == nullptr
+                                     : (n_joint >= 2 && n_joint <= gp::NB && n_joint <= m && cov != nullptr);
+  if (!joint_ok) return fail(ctx, TPE_E_INVALID, "bad joint covariance request (n_joint %d, m %lld)", n_joint,
+                             (long long)m);
+  return gp_posterior_run(ctx, params, Xq, m, 0.0, true, n_joint, mean, var, cov);
 }
 
 const char* tpe_last_logpdf_kernel(tpe_ctx* ctx) { return ctx ? ctx->last_kernel : "none"; }

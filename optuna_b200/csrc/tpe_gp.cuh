@@ -1,6 +1,7 @@
-// Gaussian-process fit of the terminator's regret bound (RegretBoundEvaluator, optuna/terminator/improvement/
-// evaluator.py:142-177): the covariance, its Cholesky factor and inverse, the negative marginal log-likelihood with its
-// gradient in the raw kernel parameters, and the posterior confidence bounds.  fp64 throughout.
+// Gaussian-process fit of the terminator's improvement evaluators (RegretBoundEvaluator, optuna/terminator/
+// improvement/evaluator.py:142-177, and EMMREvaluator, emmr.py:123-237): the covariance, its Cholesky factor and
+// inverse, the negative marginal log-likelihood with its gradient in the raw kernel parameters, and the posterior
+// (mean and variance, confidence bounds, the joint covariance of a few points).  fp64 throughout.
 //
 // Storage: n x n row-major matrices, lower triangle significant.  Two of them:
 //   A: C = ks Matern52(sum_d l_d sqd_d) + noise I (k_gp_cov), then L in place (right-looking blocked Cholesky), then
@@ -393,10 +394,12 @@ __global__ void k_gp_grad_tail(const double* __restrict__ prm, double noise_exce
 }
 
 // Per query: mean = k* . alpha (warp, fixed strides and xor tree); var = ks - sum over column tiles of the squared
-// L^-1 k* partials, in tile order, clamped at 0 (gp.py:215-250); mean +- sqrt(beta var) (acqf.py:185-214).
+// L^-1 k* partials, in tile order, clamped at 0 (gp.py:215-250).  moments: out0 = mean, out1 = var; else out0, out1 =
+// mean +- sqrt(beta var) (acqf.py:185-214).
 __global__ void k_gp_post_finish(const double* __restrict__ K, const double* __restrict__ alpha,
                                  const double* __restrict__ part, int ntiles, const double* __restrict__ prm, int P,
-                                 int n, int Q, double beta, double* __restrict__ ucb, double* __restrict__ lcb) {
+                                 int n, int Q, double beta, bool moments, double* __restrict__ out0,
+                                 double* __restrict__ out1) {
   const int qi = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
   const int lane = threadIdx.x & 31;
   if (qi >= Q) return;
@@ -409,9 +412,39 @@ __global__ void k_gp_post_finish(const double* __restrict__ K, const double* __r
     for (int b = 0; b < ntiles; ++b) s += part[(int64_t)qi * ntiles + b];
     double var = prm[P] - s;
     if (var < 0.0) var = 0.0;
-    const double h = sqrt(beta * var);
-    ucb[qi] = m + h;
-    lcb[qi] = m - h;
+    if (moments) {
+      out0[qi] = m;
+      out1[qi] = var;
+    } else {
+      const double h = sqrt(beta * var);
+      out0[qi] = m + h;
+      out1[qi] = m - h;
+    }
+  }
+}
+
+// Joint posterior covariance of the first J query points (GPRegressor.posterior with joint=True, gp.py:240-245):
+// cov[a][b] = ks Matern52(r(x_a, x_b)) - V_a . V_b with V = K L^-T (row stride n), the diagonal clamped at 0.  One
+// warp per entry: lanes strided over n, then a xor tree.  V_a . V_b and V_b . V_a are summed in the same order, so
+// the result is exactly symmetric.
+__global__ void __launch_bounds__(256) k_gp_joint_cov(const double* __restrict__ Xq, const double* __restrict__ V,
+                                                      const uint8_t* __restrict__ cat,
+                                                      const double* __restrict__ prm, int P, int n, int J,
+                                                      double* __restrict__ cov) {
+  const int e = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
+  const int lane = threadIdx.x & 31;
+  if (e >= J * J) return;
+  const int a = e / J, b = e % J;
+  const double* va = V + (int64_t)a * n;
+  const double* vb = V + (int64_t)b * n;
+  double s = 0.0;
+  for (int k = lane; k < n; k += 32) s += va[k] * vb[k];
+#pragma unroll
+  for (int o = 16; o; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
+  if (lane == 0) {
+    double c = matern52(gp_sqdist(Xq + (int64_t)a * P, Xq + (int64_t)b * P, cat, prm, P)) * prm[P] - s;
+    if (a == b && c < 0.0) c = 0.0;
+    cov[e] = c;
   }
 }
 

@@ -440,16 +440,18 @@ class TPEEngine:
         self._check(self._lib.tpe_gp_set_data(self._h, _ptr(Xa), _ptr(ya), _ptr(cat), Xa.shape[0], Xa.shape[1]))
         self._gp_P = Xa.shape[1]
 
-    def gp_loss(self, raw_params, minimum_noise: float) -> tuple[float, np.ndarray]:
+    def gp_loss(self, raw_params, minimum_noise: float, deterministic: bool = False) -> tuple[float, np.ndarray]:
         """Negative marginal log-likelihood of the GP data and its gradient in the raw kernel parameters (log
-        inverse squared lengthscales, log kernel scale, log(noise_var - minimum_noise)) (tpe_gp_loss).  Raises
-        ``GPCholeskyError`` when the covariance is not positive definite."""
+        inverse squared lengthscales, log kernel scale, log(noise_var - minimum_noise)) (tpe_gp_loss).  With
+        ``deterministic`` the noise is fixed at ``minimum_noise``, the last raw parameter is ignored and its gradient
+        is 0 (tpe_gp_loss_fixed_noise).  Raises ``GPCholeskyError`` when the covariance is not positive definite."""
         raw = _f64(raw_params)
         if self._gp_P and raw.shape != (self._gp_P + 2,):   # without GP data the library reports that first
             raise ValueError(f"raw_params must have {self._gp_P + 2} entries, got shape {raw.shape}")
         loss = C.c_double()
         grad = np.empty(raw.size)
-        self._check(self._lib.tpe_gp_loss(self._h, _ptr(raw), float(minimum_noise), C.byref(loss), _ptr(grad)))
+        fn = self._lib.tpe_gp_loss_fixed_noise if deterministic else self._lib.tpe_gp_loss
+        self._check(fn(self._h, _ptr(raw), float(minimum_noise), C.byref(loss), _ptr(grad)))
         return loss.value, grad
 
     def gp_posterior(self, params, Xq, beta: float) -> tuple[np.ndarray, np.ndarray]:
@@ -463,6 +465,21 @@ class TPEEngine:
         self._check(self._lib.tpe_gp_posterior(self._h, _ptr(prm), _ptr(xq), xq.shape[0], float(beta), _ptr(ucb),
                                                _ptr(lcb)))
         return ucb, lcb
+
+    def gp_posterior_moments(self, params, Xq, n_joint: int = 0) -> tuple[np.ndarray, np.ndarray, np.ndarray]:
+        """``(mean, var, cov)`` of the GP posterior at the rows of ``Xq`` [m, P], for ``params`` = (inverse squared
+        lengthscales, kernel scale, noise_var) (tpe_gp_posterior_moments).  ``var`` is clamped at 0.  ``cov`` is the
+        joint covariance [n_joint, n_joint] of the first ``n_joint`` rows (0, or 2 to 64), diagonal clamped at 0.
+        Raises ``GPCholeskyError`` when the covariance is not positive definite."""
+        prm, xq = _f64(params), _f64(Xq)
+        if xq.ndim != 2 or (self._gp_P and (prm.shape != (self._gp_P + 2,) or xq.shape[1] != self._gp_P)):
+            raise ValueError(f"params must have {self._gp_P + 2} entries and Xq {self._gp_P} columns")
+        n_joint = int(n_joint)
+        mean, var = np.empty(xq.shape[0]), np.empty(xq.shape[0])
+        cov = np.empty((max(n_joint, 0), max(n_joint, 0)))
+        self._check(self._lib.tpe_gp_posterior_moments(self._h, _ptr(prm), _ptr(xq), xq.shape[0], n_joint, _ptr(mean),
+                                                       _ptr(var), _ptr(cov) if n_joint else None))
+        return mean, var, cov
 
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:
