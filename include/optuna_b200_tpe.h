@@ -40,7 +40,8 @@ extern "C" {
 /* 9: + tpe_fanova_variances */
 /* 10: + tpe_gp_set_data, tpe_gp_loss, tpe_gp_posterior, TPE_E_NOTPD */
 /* 11: + tpe_gp_loss_fixed_noise, tpe_gp_posterior_moments */
-#define TPE_ABI_VERSION 11
+/* 12: + tpe_gp_condition, tpe_gp_query */
+#define TPE_ABI_VERSION 12
 
 enum {
   TPE_OK = 0,
@@ -296,8 +297,8 @@ int tpe_fanova_variances(tpe_ctx* ctx, int32_t n_trees, const int64_t* node_offs
                          int32_t n_features, const double* bounds, int32_t n_params, const int32_t* param_offsets,
                          const int32_t* raw_features, double* tree_variance, double* marginal_variance);
 /* Gaussian process of the terminator's improvement evaluators (RegretBoundEvaluator, optuna/terminator/improvement/
- * evaluator.py:142-177, and EMMREvaluator, emmr.py:123-237), fp64.  Kept apart from the history and the suggestion
- * state.
+ * evaluator.py:142-177, and EMMREvaluator, emmr.py:123-237) and of GPSampler (optuna/samplers/_gp/sampler.py), fp64.
+ * Kept apart from the history and the suggestion state.
  * tpe_gp_set_data replaces the GPRegressor's training data (optuna/_gp/gp.py:94-118): X [n, P] normalised
  * parameters, y [n] standardised values, is_categorical [P] (0 / 1); n >= 1, P >= 1, all finite.  Allocates two
  * n x n matrices; TPE_E_INVALID naming the need when the device lacks the memory.
@@ -313,6 +314,14 @@ int tpe_fanova_variances(tpe_ctx* ctx, int32_t n_trees, const int64_t* node_offs
  * 0; with n_joint in [2, 64] (and <= m) also the joint covariance of the first n_joint points, cov [n_joint *
  * n_joint] row-major, diagonal clamped at 0 (joint=True); n_joint = 0 and cov = NULL for none.  One factorisation
  * per call.
+ * tpe_gp_condition replaces GPRegressor._cache_matrix (gp.py:124-149) and, after a new tpe_gp_set_data of the train
+ * and running rows, append_running_data (gp.py:151-183): it factorises once at params [P + 2] and keeps L^-1 and
+ * C^-1 y for tpe_gp_query.  tpe_gp_set_data, the loss calls and the posterior calls overwrite that factor and undo it.
+ * tpe_gp_query replaces GPRegressor.posterior (gp.py:215-250, joint=False) and its autograd backward in x, as the
+ * acquisition functions of optuna/_gp/acqf.py and optim_mixed.optimize_acqf_mixed call it: at m query rows Xq [m, P],
+ * mean [m] and var [m] clamped at 0 against the conditioned factor, with no refactorisation; with dmean and dvar
+ * non-NULL also their gradients in x, [m, P] each, 0 in categorical columns and, for dvar, where var was clamped.  The
+ * values do not depend on whether gradients are asked for.  TPE_E_STATE when the context is not conditioned.
  * All return TPE_E_NOTPD when a Cholesky pivot is <= 0 or NaN; the loss calls also when a raw parameter they read is
  * NaN or large enough that a kernel parameter is not finite (the reference's Cholesky fails there too). */
 int tpe_gp_set_data(tpe_ctx* ctx, const double* X, const double* y, const uint8_t* is_categorical, int64_t n,
@@ -323,6 +332,8 @@ int tpe_gp_posterior(tpe_ctx* ctx, const double* params, const double* Xq, int64
 int tpe_gp_loss_fixed_noise(tpe_ctx* ctx, const double* raw, double noise_var, double* loss, double* grad);
 int tpe_gp_posterior_moments(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, int32_t n_joint,
                              double* mean, double* var, double* cov);
+int tpe_gp_condition(tpe_ctx* ctx, const double* params);
+int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double* var, double* dmean, double* dvar);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

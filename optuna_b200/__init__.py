@@ -8,7 +8,7 @@ from .engine import ParamSpec, TPEEngine  # noqa: F401
 
 __all__ = ["ParamSpec", "TPEEngine", "B200TPESampler", "hypervolume_history", "plot_hypervolume_history",
            "best_trials", "pareto_front_info", "plot_pareto_front", "FanovaImportanceEvaluator",
-           "RegretBoundEvaluator", "EMMREvaluator"]
+           "RegretBoundEvaluator", "EMMREvaluator", "GPSampler"]
 
 
 def __getattr__(name):
@@ -25,4 +25,7 @@ def __getattr__(name):
     if name in ("RegretBoundEvaluator", "EMMREvaluator"):
         from . import terminator
         return getattr(terminator, name)
+    if name == "GPSampler":
+        from .gp_sampler import GPSampler
+        return GPSampler
     raise AttributeError(name)

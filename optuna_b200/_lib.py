@@ -79,6 +79,8 @@ SYMBOLS = {
     "tpe_gp_posterior": (C.c_int, [_P, _P, _P, C.c_int64, C.c_double, _P, _P]),
     "tpe_gp_loss_fixed_noise": (C.c_int, [_P, _P, C.c_double, C.POINTER(C.c_double), _P]),
     "tpe_gp_posterior_moments": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int32, _P, _P, _P]),
+    "tpe_gp_condition": (C.c_int, [_P, _P]),
+    "tpe_gp_query": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P, _P]),
     "tpe_get_candidates": (C.c_int, [_P, _P, _P, _P]),
     "tpe_logpdf": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P]),
     "tpe_last_timing": (C.c_int, [_P, _P, _P]),
@@ -89,7 +91,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 11  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 12  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

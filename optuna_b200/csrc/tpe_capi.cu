@@ -120,14 +120,16 @@ struct GpState {
   int32_t P = 0;
   double *X = nullptr, *y = nullptr, *A = nullptr, *B = nullptr, *W = nullptr, *u = nullptr, *alpha = nullptr;
   double *prm = nullptr, *part = nullptr, *scal = nullptr, *grad = nullptr, *Xq = nullptr, *ucb = nullptr,
-         *lcb = nullptr;
+         *lcb = nullptr, *dmean = nullptr, *dvar = nullptr;
   uint8_t* cat = nullptr;
   int* fail = nullptr;
   int64_t part_cap = 0, xq_cap = 0;
-  bool ready = false;   // tpe_gp_set_data completed: every buffer above is allocated
+  bool ready = false;         // tpe_gp_set_data completed: every buffer above is allocated
+  bool conditioned = false;   // B, alpha and prm hold the factor of tpe_gp_condition: tpe_gp_query may read them
   void release() {
     for (void* p : {(void*)X, (void*)y, (void*)A, (void*)B, (void*)W, (void*)u, (void*)alpha, (void*)prm, (void*)part,
-                    (void*)scal, (void*)grad, (void*)Xq, (void*)ucb, (void*)lcb, (void*)cat, (void*)fail})
+                    (void*)scal, (void*)grad, (void*)Xq, (void*)ucb, (void*)lcb, (void*)dmean, (void*)dvar,
+                    (void*)cat, (void*)fail})
       if (p) cudaFree(p);
     *this = GpState();
   }
@@ -3589,6 +3591,7 @@ int tpe_gp_set_data(tpe_ctx* ctx, const double* X, const double* y, const uint8_
                     int32_t P) {
   if (!ctx) return TPE_E_INVALID;
   std::lock_guard<std::mutex> lk(ctx->mu);
+  ctx->gp.conditioned = false;
   if (n < 1 || P < 1 || n > (int64_t)1 << 30) return fail(ctx, TPE_E_INVALID, "bad GP sizes (n %lld, P %d)", (long long)n, P);
   if (!X || !y || !is_categorical) return fail(ctx, TPE_E_INVALID, "bad GP arguments");
   for (int64_t i = 0; i < n * P; ++i)
@@ -3602,7 +3605,8 @@ int tpe_gp_set_data(tpe_ctx* ctx, const double* X, const double* y, const uint8_
   const int64_t part = std::max<int64_t>(npass * kGpGradBlocks * (gp::GRAD_DC + 2), kGpQmax * ((n + gp::NB - 1) / gp::NB));
   const size_t a_elems = (size_t)std::max<int64_t>(n, kGpQmax) * n, b_elems = (size_t)n * n;
   // A, B, the TRTRI panel, X / y / u / alpha, the partial sums and scalars, and the posterior's query buffers for
-  // the evaluator's n + 2048 points (Xq, ucb, lcb)
+  // the evaluator's n + 2048 points (Xq, ucb, lcb).  The gradient buffers of tpe_gp_query are allocated and checked
+  // by the first query that asks for gradients.
   const size_t n_query = (size_t)n + 2048;
   const size_t need = 8 * (a_elems + b_elems + (size_t)n * gp::NB + (size_t)n * (P + 3) + (size_t)part + 3 * (P + 2) +
                            2 + n_query * (P + 2)) + P + sizeof(int);
@@ -3631,6 +3635,7 @@ static int gp_loss_run(tpe_ctx* ctx, const double* raw, double noise_excess, dou
                        double* grad) {
   GpState& g = ctx->gp;
   const int P = g.P;
+  g.conditioned = false;   // B and prm are overwritten
   if (set_device(ctx)) return TPE_E_CUDA;
   std::vector<double> prm(P + 2);
   for (int d = 0; d < P; ++d) prm[d] = std::exp(raw[d]);
@@ -3691,39 +3696,74 @@ int tpe_gp_loss_fixed_noise(tpe_ctx* ctx, const double* raw, double noise_var, d
   return gp_loss_run(ctx, raw, 0.0, noise_var, loss, grad);
 }
 
-// The body of tpe_gp_posterior and tpe_gp_posterior_moments, called under the context lock with the arguments
-// checked: factorise at params, then per chunk of query rows the cross covariance, the squared norms of L^-1 k* and
-// k_gp_post_finish (moments: mean / var, else mean +- sqrt(beta var)).  With J > 0 also the joint covariance of the
-// first J query rows into cov [J * J].
-static int gp_posterior_run(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta,
-                            bool moments, int J, double* out0, double* out1, double* cov) {
+// Query buffers for m rows: Xq and the two value outputs (ucb / lcb, or mean / var)
+static int gp_query_buffers(tpe_ctx* ctx, int64_t m) {
   GpState& g = ctx->gp;
-  const int P = g.P;
-  if (set_device(ctx)) return TPE_E_CUDA;
-  cudaStream_t st = ctx->stream;
-  if (m > g.xq_cap) {
-    for (double** p : {&g.Xq, &g.ucb, &g.lcb}) {
-      if (*p) cudaFree(*p);
-      *p = nullptr;
-    }
-    g.xq_cap = 0;
-    CU(cudaMalloc(&g.Xq, (size_t)m * P * 8));
-    CU(cudaMalloc(&g.ucb, m * 8));
-    CU(cudaMalloc(&g.lcb, m * 8));
-    g.xq_cap = m;
+  if (m <= g.xq_cap) return TPE_OK;
+  for (double** p : {&g.Xq, &g.ucb, &g.lcb}) {
+    if (*p) cudaFree(*p);
+    *p = nullptr;
   }
-  CU(cudaMemcpyAsync(g.prm, params, (P + 2) * 8, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(g.Xq, Xq, (size_t)m * P * 8, cudaMemcpyHostToDevice, st));
-  gp_factor(ctx);
-  const int64_t n = g.n, ntiles = (n + gp::NB - 1) / gp::NB;
-  for (int64_t q0 = 0; q0 < m; q0 += kGpQmax) {
-    const int64_t Q = std::min(kGpQmax, m - q0);
+  g.xq_cap = 0;
+  CU(cudaMalloc(&g.Xq, (size_t)m * g.P * 8));
+  CU(cudaMalloc(&g.ucb, m * 8));
+  CU(cudaMalloc(&g.lcb, m * 8));
+  g.xq_cap = m;
+  return TPE_OK;
+}
+
+// The gradient outputs of one query chunk (NB rows x P each), allocated by the first query that asks for gradients:
+// the posterior calls never touch them
+static int gp_grad_buffers(tpe_ctx* ctx) {
+  GpState& g = ctx->gp;
+  if (g.dmean) return TPE_OK;
+  const size_t bytes = (size_t)gp::NB * g.P * 8;
+  size_t free_b = 0, total_b = 0;
+  CU(cudaMemGetInfo(&free_b, &total_b));
+  if (2 * bytes > free_b)
+    return fail(ctx, TPE_E_INVALID, "the GP posterior gradient needs %zu bytes of device memory, device %d has %zu free",
+                2 * bytes, ctx->device, free_b);
+  if (g.dvar) cudaFree(g.dvar);   // left by an earlier call whose second allocation failed
+  g.dvar = nullptr;
+  CU(cudaMalloc(&g.dvar, bytes));   // dvar first: dmean != nullptr marks both allocated
+  CU(cudaMalloc(&g.dmean, bytes));
+  return TPE_OK;
+}
+
+// The query rows of g.Xq against the factor in B, alpha and prm (A is scratch).  Per chunk of rows (kGpQmax, or NB
+// with grad): the cross covariance into A, the squared norms of L^-1 k* and k_gp_post_finish (moments: mean / var
+// into ucb / lcb, else mean +- sqrt(beta var)).  Every row's values depend on that row alone, so they are the same
+// whatever the chunk size.  With host gradient outputs dmean_h / dvar_h [m, P] (both or neither) also V = K L^-T into
+// the n x 64 TRTRI panel (free after gp_factor), Wm = V L^-1 into rows NB .. 2 NB - 1 of A, k_gp_post_grad into the
+// chunk's gradient buffers, and their copy to the host.  V repeats the O(Q n^2) product of the squared norms: the
+// values must not depend on whether gradients are asked for, so they come from the same kernels either way.  With
+// J > 0 the joint covariance of the first J rows into part [J * J].
+static int gp_query_chunks(tpe_ctx* ctx, int64_t m, double beta, bool moments, int J, double* dmean_h,
+                           double* dvar_h) {
+  GpState& g = ctx->gp;
+  cudaStream_t st = ctx->stream;
+  const int P = g.P;
+  const bool grad = dmean_h != nullptr;
+  const int64_t n = g.n, ntiles = (n + gp::NB - 1) / gp::NB, qmax = grad ? gp::NB : kGpQmax;
+  double* Wm = g.A + gp::NB * n;   // A has at least kGpQmax >= 2 NB rows of n
+  for (int64_t q0 = 0; q0 < m; q0 += qmax) {
+    const int64_t Q = std::min(qmax, m - q0);
     gp::k_gp_cross<<<dim3((unsigned)((n + 127) / 128), (unsigned)Q), 128, 0, st>>>(g.Xq + q0 * P, g.X, g.cat, g.prm,
                                                                                   P, (int)n, (int)Q, g.A);
     // squared norms of L^-1 k*, per query and column tile
     gp_gemm(st, g.A, n, g.B, n, g.part, 0, Q, n, n, 1.0, gp::GF_KHI_COL | gp::GF_SQSUM);
     gp::k_gp_post_finish<<<(unsigned)((Q + 7) / 8), 256, 0, st>>>(g.A, g.alpha, g.part, (int)ntiles, g.prm, P, (int)n,
                                                                   (int)Q, beta, moments, g.ucb + q0, g.lcb + q0);
+    if (grad) {
+      gp_gemm(st, g.A, n, g.B, n, g.W, n, Q, n, n, 1.0, gp::GF_KHI_COL);
+      gp_gemm(st, g.W, n, g.B, n, Wm, n, Q, n, n, 1.0, gp::GF_TB | gp::GF_KLO_COL);
+      const dim3 grid((unsigned)Q, (unsigned)((P + gp::GRAD_DC - 1) / gp::GRAD_DC));
+      gp::k_gp_post_grad<gp::GRAD_DC><<<grid, gp::GRAD_THREADS, 0, st>>>(
+          g.Xq + q0 * P, g.X, g.cat, g.prm, g.alpha, Wm, g.part, (int)ntiles, P, (int)n, g.dmean, g.dvar);
+      // stream order: the next chunk's k_gp_post_grad writes the buffers after these copies have read them
+      CU(cudaMemcpyAsync(dmean_h + q0 * P, g.dmean, (size_t)Q * P * 8, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(dvar_h + q0 * P, g.dvar, (size_t)Q * P * 8, cudaMemcpyDeviceToHost, st));
+    }
     if (q0 == 0 && J > 0) {
       // V = K L^-T for the first J rows (J <= min(m, 64), so all in this chunk) into the n x 64 TRTRI panel
       // buffer, free after gp_factor
@@ -3732,6 +3772,25 @@ static int gp_posterior_run(tpe_ctx* ctx, const double* params, const double* Xq
   }
   if (J > 0)   // after the last chunk's k_gp_post_finish has read g.part (>= 18 432 entries, see tpe_gp_set_data)
     gp::k_gp_joint_cov<<<(unsigned)((J * J + 7) / 8), 256, 0, st>>>(g.Xq, g.W, g.cat, g.prm, P, (int)n, J, g.part);
+  return TPE_OK;
+}
+
+// The body of tpe_gp_posterior and tpe_gp_posterior_moments, called under the context lock with the arguments
+// checked: factorise at params, then gp_query_chunks.  The factor in B is this call's: tpe_gp_query needs a new
+// tpe_gp_condition.
+static int gp_posterior_run(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, double beta,
+                            bool moments, int J, double* out0, double* out1, double* cov) {
+  GpState& g = ctx->gp;
+  const int P = g.P;
+  g.conditioned = false;
+  if (set_device(ctx)) return TPE_E_CUDA;
+  cudaStream_t st = ctx->stream;
+  const int rc = gp_query_buffers(ctx, m);
+  if (rc != TPE_OK) return rc;
+  CU(cudaMemcpyAsync(g.prm, params, (P + 2) * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(g.Xq, Xq, (size_t)m * P * 8, cudaMemcpyHostToDevice, st));
+  gp_factor(ctx);
+  gp_query_chunks(ctx, m, beta, moments, J, nullptr, nullptr);   // without gradients it makes no call that can fail
   CU(cudaGetLastError());
   int failed = 0;
   CU(cudaMemcpyAsync(&failed, g.fail, sizeof(int), cudaMemcpyDeviceToHost, st));
@@ -3743,16 +3802,25 @@ static int gp_posterior_run(tpe_ctx* ctx, const double* params, const double* Xq
   return TPE_OK;
 }
 
+static int gp_params_check(tpe_ctx* ctx, const double* params) {
+  for (int d = 0; d < ctx->gp.P + 2; ++d)
+    if (!std::isfinite(params[d])) return fail(ctx, TPE_E_INVALID, "kernel parameters hold a non-finite value");
+  return TPE_OK;
+}
+
+static int gp_xq_check(tpe_ctx* ctx, const double* Xq, int64_t m) {
+  for (int64_t i = 0; i < m * ctx->gp.P; ++i)
+    if (!std::isfinite(Xq[i])) return fail(ctx, TPE_E_INVALID, "query points hold a non-finite value");
+  return TPE_OK;
+}
+
 // the argument checks the two posterior entry points share
 static int gp_posterior_check(tpe_ctx* ctx, const double* params, const double* Xq, int64_t m, bool ok) {
   GpState& g = ctx->gp;
   if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
   if (!params || !Xq || !ok || m < 1) return fail(ctx, TPE_E_INVALID, "bad GP posterior arguments");
-  for (int d = 0; d < g.P + 2; ++d)
-    if (!std::isfinite(params[d])) return fail(ctx, TPE_E_INVALID, "kernel parameters hold a non-finite value");
-  for (int64_t i = 0; i < m * g.P; ++i)
-    if (!std::isfinite(Xq[i])) return fail(ctx, TPE_E_INVALID, "query points hold a non-finite value");
-  return TPE_OK;
+  const int rc = gp_params_check(ctx, params);
+  return rc != TPE_OK ? rc : gp_xq_check(ctx, Xq, m);
 }
 
 // replaces GPRegressor._cache_matrix + posterior (optuna/_gp/gp.py:124-149, 215-250) and UCB / LCB.eval_acqf
@@ -3780,6 +3848,58 @@ int tpe_gp_posterior_moments(tpe_ctx* ctx, const double* params, const double* X
   if (!joint_ok) return fail(ctx, TPE_E_INVALID, "bad joint covariance request (n_joint %d, m %lld)", n_joint,
                              (long long)m);
   return gp_posterior_run(ctx, params, Xq, m, 0.0, true, n_joint, mean, var, cov);
+}
+
+// replaces GPRegressor._cache_matrix (gp.py:124-149): factorise once at params and keep L^-1 and alpha for
+// tpe_gp_query
+int tpe_gp_condition(tpe_ctx* ctx, const double* params) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  GpState& g = ctx->gp;
+  if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
+  if (!params) return fail(ctx, TPE_E_INVALID, "bad GP condition arguments");
+  const int rc = gp_params_check(ctx, params);
+  if (rc != TPE_OK) return rc;
+  g.conditioned = false;
+  if (set_device(ctx)) return TPE_E_CUDA;
+  cudaStream_t st = ctx->stream;
+  CU(cudaMemcpyAsync(g.prm, params, (g.P + 2) * 8, cudaMemcpyHostToDevice, st));
+  gp_factor(ctx);
+  CU(cudaGetLastError());
+  int failed = 0;
+  CU(cudaMemcpyAsync(&failed, g.fail, sizeof(int), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (failed) return fail(ctx, TPE_E_NOTPD, "the GP covariance is not positive definite (Cholesky pivot <= 0 or NaN)");
+  g.conditioned = true;
+  return TPE_OK;
+}
+
+// replaces GPRegressor.posterior (gp.py:215-250) and its autograd backward in x, against the factor of
+// tpe_gp_condition: mean and var at m query points and, with dmean / dvar, their gradients in the query point
+int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double* var, double* dmean,
+                 double* dvar) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  GpState& g = ctx->gp;
+  if (!g.ready) return fail(ctx, TPE_E_STATE, "no GP data (tpe_gp_set_data)");
+  if (!g.conditioned) return fail(ctx, TPE_E_STATE, "the GP is not conditioned (tpe_gp_condition)");
+  if (!Xq || !mean || !var || m < 1 || (dmean == nullptr) != (dvar == nullptr))
+    return fail(ctx, TPE_E_INVALID, "bad GP query arguments");
+  int rc = gp_xq_check(ctx, Xq, m);
+  if (rc != TPE_OK) return rc;
+  if (set_device(ctx)) return TPE_E_CUDA;
+  rc = gp_query_buffers(ctx, m);
+  if (rc == TPE_OK && dmean) rc = gp_grad_buffers(ctx);
+  if (rc != TPE_OK) return rc;
+  cudaStream_t st = ctx->stream;
+  CU(cudaMemcpyAsync(g.Xq, Xq, (size_t)m * g.P * 8, cudaMemcpyHostToDevice, st));
+  rc = gp_query_chunks(ctx, m, 0.0, true, 0, dmean, dvar);
+  if (rc != TPE_OK) return rc;
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(mean, g.ucb, m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(var, g.lcb, m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
 }
 
 const char* tpe_last_logpdf_kernel(tpe_ctx* ctx) { return ctx ? ctx->last_kernel : "none"; }

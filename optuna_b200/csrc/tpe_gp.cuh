@@ -1,11 +1,14 @@
 // Gaussian-process fit of the terminator's improvement evaluators (RegretBoundEvaluator, optuna/terminator/
 // improvement/evaluator.py:142-177, and EMMREvaluator, emmr.py:123-237): the covariance, its Cholesky factor and
 // inverse, the negative marginal log-likelihood with its gradient in the raw kernel parameters, and the posterior
-// (mean and variance, confidence bounds, the joint covariance of a few points).  fp64 throughout.
+// (mean and variance, confidence bounds, the joint covariance of a few points).  GPSampler (optuna/samplers/_gp/
+// sampler.py) conditions once and then queries the posterior and its gradient in the query point many times against
+// the kept L^-1 and alpha.  fp64 throughout.
 //
 // Storage: n x n row-major matrices, lower triangle significant.  Two of them:
 //   A: C = ks Matern52(sum_d l_d sqd_d) + noise I (k_gp_cov), then L in place (right-looking blocked Cholesky), then
-//      C^-1 = L^-T L^-1 (k_gp_gemm, lower triangle); during the posterior, the query-by-train cross covariance.
+//      C^-1 = L^-T L^-1 (k_gp_gemm, lower triangle); during the posterior, the query-by-train cross covariance (and,
+//      for gradients, C^-1 k* = L^-T L^-1 k* in rows 64 .. 127).
 //   B: L^-1 (blocked TRTRI); upper triangle zero.
 // Every O(n^3) step -- the trailing SYRK, the panel TRSM (against the inverted diagonal block), the TRMM of the
 // TRTRI, the L^-T L^-1 product and L^-1 k* of the posterior -- is one k_gp_gemm: 64 x 64 tiles on mma.m16n8k8.f64.
@@ -133,6 +136,7 @@ constexpr int GF_KHI_ROW = 16;  // k ends at the tile's last row (opA zero for k
 constexpr int GF_KHI_COL = 32;  // k ends at the tile's last column (opB zero for k > j)
 constexpr int GF_SQSUM = 64;    // no store: part[i * gridDim.x + bx] = sum over the tile's columns of out(i, j)^2
 constexpr int GF_ACCUM = 128;   // out = alpha * acc + out (else out = alpha * acc)
+constexpr int GF_KLO_COL = 256; // k starts at the tile's first column (opB zero for k < j)
 
 // out(i, j) = alpha sum_k opA(i, k) opB(j, k) over an M x N output in 64 x 64 tiles, 4 warps of 32 x 32, each warp
 // 2 x 4 fragments of mma.m16n8k8.f64.  A CTA reads all its operand rows before it writes: out may alias the rows of
@@ -148,6 +152,7 @@ __global__ void __launch_bounds__(128) k_gp_gemm(const double* A, int64_t lda, c
   __shared__ double red[2][NB];
   int kb = 0, ke = K;
   if (flags & GF_KLO_ROW) kb = i0;
+  if (flags & GF_KLO_COL) kb = j0;
   if (flags & GF_KHI_ROW) ke = min(ke, i0 + NB);
   if (flags & GF_KHI_COL) ke = min(ke, j0 + NB);
   kb = (kb / GK) * GK;
@@ -420,6 +425,76 @@ __global__ void k_gp_post_finish(const double* __restrict__ K, const double* __r
       out0[qi] = m + h;
       out1[qi] = m - h;
     }
+  }
+}
+
+// Gradients of the posterior mean and variance in the query point (GPRegressor.posterior under autograd, gp.py:
+// 215-250, with the Matern derivative saved by gp.py:63-90):
+//   dmean/dx_d = 2 l_d ks sum_i alpha_i M'(r_i) (x_d - X_id)
+//   dvar/dx_d  = -2 (2 l_d ks sum_i w_i M'(r_i) (x_d - X_id)),   w = C^-1 k* (row q of Wm, row stride n)
+// Both are 0 in a categorical column (the reference's `> 0` passes no gradient), and dvar is 0 where the raw variance
+// (ks minus the partials of part summed in k_gp_post_finish's order) was clamped.  One CTA per (query, DC columns):
+// threads strided over the n training rows, then a xor tree and the warps in order; no atomics.
+template <int DC>
+__global__ void __launch_bounds__(GRAD_THREADS) k_gp_post_grad(const double* __restrict__ Xq,
+                                                               const double* __restrict__ X,
+                                                               const uint8_t* __restrict__ cat,
+                                                               const double* __restrict__ prm,
+                                                               const double* __restrict__ alpha,
+                                                               const double* __restrict__ Wm,
+                                                               const double* __restrict__ part, int ntiles, int P,
+                                                               int n, double* __restrict__ dmean,
+                                                               double* __restrict__ dvar) {
+  __shared__ double red[GRAD_THREADS / 32][2 * DC];
+  const int q = blockIdx.x, d0 = blockIdx.y * DC;
+  const int dn = min(DC, P - d0);
+  const double* xq = Xq + (int64_t)q * P;
+  const double* wq = Wm + (int64_t)q * n;
+  double am[DC], av[DC];
+#pragma unroll
+  for (int s = 0; s < DC; ++s) am[s] = av[s] = 0.0;
+  for (int i = threadIdx.x; i < n; i += GRAD_THREADS) {
+    const double* xi = X + (int64_t)i * P;
+    double val, der;
+    matern52_both(gp_sqdist(xq, xi, cat, prm, P), val, der);
+    const double cm = alpha[i] * der, cv = wq[i] * der;
+#pragma unroll
+    for (int s = 0; s < DC; ++s) {
+      if (s < dn) {
+        const double t = xq[d0 + s] - xi[d0 + s];
+        am[s] += cm * t;
+        av[s] += cv * t;
+      }
+    }
+  }
+  const int lane = threadIdx.x & 31, wp = threadIdx.x >> 5;
+#pragma unroll
+  for (int s = 0; s < DC; ++s) {
+    double a = am[s], b = av[s];
+#pragma unroll
+    for (int o = 16; o; o >>= 1) {
+      a += __shfl_xor_sync(0xffffffffu, a, o);
+      b += __shfl_xor_sync(0xffffffffu, b, o);
+    }
+    if (lane == 0) {
+      red[wp][s] = a;
+      red[wp][DC + s] = b;
+    }
+  }
+  __syncthreads();
+  if (threadIdx.x < dn) {
+    const int s = threadIdx.x, d = d0 + s;
+    double vm = red[0][s], vv = red[0][DC + s];
+    for (int k = 1; k < GRAD_THREADS / 32; ++k) {
+      vm += red[k][s];
+      vv += red[k][DC + s];
+    }
+    double sq = 0.0;
+    for (int b = 0; b < ntiles; ++b) sq += part[(int64_t)q * ntiles + b];
+    const bool clamped = prm[P] - sq < 0.0;
+    const double l2 = 2.0 * prm[d] * prm[P];
+    dmean[(int64_t)q * P + d] = cat[d] ? 0.0 : l2 * vm;
+    dvar[(int64_t)q * P + d] = (cat[d] || clamped) ? 0.0 : -2.0 * (l2 * vv);
   }
 }
 

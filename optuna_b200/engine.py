@@ -481,6 +481,29 @@ class TPEEngine:
                                                        _ptr(var), _ptr(cov) if n_joint else None))
         return mean, var, cov
 
+    def gp_condition(self, params) -> None:
+        """Factorise the GP covariance once at ``params`` = (inverse squared lengthscales, kernel scale, noise_var) and
+        keep the factor for ``gp_query`` (tpe_gp_condition).  ``gp_set_data``, ``gp_loss`` and the posterior calls
+        undo it.  Raises ``GPCholeskyError`` when the covariance is not positive definite."""
+        prm = _f64(params)
+        if self._gp_P and prm.shape != (self._gp_P + 2,):
+            raise ValueError(f"params must have {self._gp_P + 2} entries, got shape {prm.shape}")
+        self._check(self._lib.tpe_gp_condition(self._h, _ptr(prm)))
+
+    def gp_query(self, Xq, grad: bool = False):
+        """The GP posterior at the rows of ``Xq`` [m, P] against the factor of ``gp_condition`` (tpe_gp_query):
+        ``(mean, var)``, ``var`` clamped at 0, and with ``grad`` also ``(dmean, dvar)`` [m, P], their gradients in the
+        query point.  The values are the same bits with and without ``grad``."""
+        xq = _f64(Xq)
+        if xq.ndim != 2 or (self._gp_P and xq.shape[1] != self._gp_P):
+            raise ValueError(f"Xq must be [m, {self._gp_P}], got shape {xq.shape}")
+        mean, var = np.empty(xq.shape[0]), np.empty(xq.shape[0])
+        dmean = np.empty(xq.shape) if grad else None
+        dvar = np.empty(xq.shape) if grad else None
+        self._check(self._lib.tpe_gp_query(self._h, _ptr(xq), xq.shape[0], _ptr(mean), _ptr(var), _ptr(dmean),
+                                           _ptr(dvar)))
+        return (mean, var, dmean, dvar) if grad else (mean, var)
+
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:
         below = np.empty(self._info[1], dtype=np.int64)

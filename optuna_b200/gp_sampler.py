@@ -1,0 +1,268 @@
+"""optuna's Bayesian-optimisation sampler with its Gaussian processes on the GPU: a drop-in ``GPSampler``.
+
+``optuna.samplers.GPSampler`` does two costly things per trial (optuna/samplers/_gp/sampler.py:358-485):
+- it fits one Gaussian process per objective and one per constraint by L-BFGS-B over the kernel parameters; every
+  loss evaluation builds an n x n x P tensor and runs autograd through a Cholesky factor (optuna/_gp/gp.py:287-409);
+- it maximises the acquisition function (optuna/_gp/optim_mixed.py): 2 048 QMC points, then up to 10 local searches
+  of L-BFGS-B and discrete steps.  Every evaluation calls ``GPRegressor.posterior``, two triangular solves against the
+  n x n factor plus torch autograd for the gradient in x.
+
+This sampler subclasses optuna's and keeps every host step: the standardisation, the cache handling, the choice of
+starting points, the random stream, optuna's acquisition functions and ``optimize_acqf_mixed``.  Only the GPs move to
+the device.  Each GP is fitted by the terminator's device fit (``terminator._fit``: the loss and its gradient on the
+device, scipy's L-BFGS-B and the prior on the host), factorised once, and queried with its posterior and the
+posterior's gradient in x against that factor (``TPEEngine.gp_condition`` / ``gp_query``).
+
+One difference: the device holds two n x n fp64 matrices per GP, and ``sample_relative`` raises ``ValueError``
+naming the need when the device lacks that memory.
+"""
+from __future__ import annotations
+
+import threading
+from typing import Any
+
+import numpy as np
+import torch
+from optuna._gp import acqf as acqf_module
+from optuna._gp import search_space as gp_search_space
+from optuna.samplers import GPSampler as _OptunaGPSampler
+from optuna.samplers._gp.sampler import EPS, _get_constraint_vals_and_feasibility, _standardize_values
+from optuna.study import StudyDirection
+
+from .engine import GPCholeskyError, TPEEngine
+from .terminator import _fit
+
+# the engine class that answers the computation (tests substitute a host implementation)
+_engine_cls = TPEEngine
+
+
+def _condition(engine, params: np.ndarray) -> None:
+    try:
+        engine.gp_condition(params)
+    except GPCholeskyError as e:
+        # the reference factorises the final covariance with NumPy (gp.py:132)
+        raise np.linalg.LinAlgError("Matrix is not positive definite") from e
+
+
+class _Posterior(torch.autograd.Function):
+    """``GPRegressor.posterior(x)`` (gp.py:215-250) from one device query; the backward is
+    ``g_mean dmean/dx + g_var dvar/dx`` with the gradients that query returned."""
+
+    @staticmethod
+    def forward(ctx: Any, x: torch.Tensor, gpr: _DeviceGP) -> tuple[torch.Tensor, torch.Tensor]:
+        want_grad = ctx.needs_input_grad[0]
+        xs = x.detach().cpu().numpy().reshape(-1, x.shape[-1])
+        out = gpr._engine.gp_query(xs, grad=want_grad)
+        if want_grad:
+            ctx.save_for_backward(torch.from_numpy(out[2]).reshape(x.shape), torch.from_numpy(out[3]).reshape(x.shape))
+        return torch.from_numpy(out[0]).reshape(x.shape[:-1]), torch.from_numpy(out[1]).reshape(x.shape[:-1])
+
+    @staticmethod
+    def backward(ctx: Any, g_mean: torch.Tensor, g_var: torch.Tensor) -> tuple[torch.Tensor, None]:
+        dmean, dvar = ctx.saved_tensors
+        return g_mean[..., None] * dmean + g_var[..., None] * dvar, None
+
+
+class _DeviceGP:
+    """What optuna's acquisition functions (optuna/_gp/acqf.py) and ``GPSampler`` read of a fitted ``GPRegressor``,
+    answered by an engine conditioned at the fitted parameters."""
+
+    def __init__(self, engine, X: np.ndarray, y: np.ndarray, is_categorical: np.ndarray, params: np.ndarray) -> None:
+        P = X.shape[1]
+        self._engine = engine
+        self._X_train, self._is_categorical, self._params = X, is_categorical, params
+        self._y_train = torch.from_numpy(y)
+        self.inverse_squared_lengthscales = torch.from_numpy(params[:P].copy())
+        self.kernel_scale = torch.tensor(params[P], dtype=torch.float64)
+        self.noise_var = torch.tensor(params[P + 1], dtype=torch.float64)
+        _condition(engine, params)
+
+    @property
+    def length_scales(self) -> np.ndarray:
+        return 1.0 / np.sqrt(self.inverse_squared_lengthscales.detach().cpu().numpy())
+
+    def append_running_data(self, X_running: torch.Tensor, y_running: torch.Tensor) -> None:
+        # gp.py:151-183 extends the factor block-wise; the factor of the stacked train and running rows at the same
+        # parameters is of the same matrix
+        X = np.concatenate([self._X_train, X_running.detach().cpu().numpy()])
+        y = np.concatenate([self._y_train.numpy(), y_running.detach().cpu().numpy()])
+        self._engine.gp_set_data(X, y, self._is_categorical)
+        _condition(self._engine, self._params)
+
+    def posterior(self, x: torch.Tensor, joint: bool = False) -> tuple[torch.Tensor, torch.Tensor]:
+        if joint:
+            raise NotImplementedError("GPSampler's acquisition functions do not ask for the joint posterior")
+        return _Posterior.apply(x, self)
+
+
+class GPSampler(_OptunaGPSampler):
+    """Gaussian-process Bayesian-optimisation sampler whose Gaussian processes are fitted and queried on the GPU.
+
+    A drop-in for ``optuna.samplers.GPSampler`` with the same arguments and ``device``.  For the same seed and history
+    it consumes the random stream as the reference does and suggests the reference's parameters, up to the rounding
+    of the device's fp64 sums.  Its engines (one per objective and per constraint) are kept across trials; ``close``
+    frees them.  Under ``study.optimize(n_jobs > 1)`` the relative sampling of concurrent trials runs one at a time,
+    since the trials share those engines.
+
+    The device holds two n x n fp64 matrices per GP, n being the number of complete trials (plus the running ones in a
+    single-objective study without constraints).  When it lacks that memory, ``sample_relative`` raises
+    ``ValueError`` naming the need; this is the one difference from the reference.
+
+    Args:
+        seed: Random seed.
+        independent_sampler: Sampler for the startup trials and for conditional parameters.
+        n_startup_trials: Number of initial trials.
+        deterministic_objective: Whether the objective function is deterministic (the GP noise is then fixed at its
+            minimum).
+        constraints_func: A function that computes the constraints of a trial.
+        warn_independent_sampling: Whether to warn when a parameter is sampled by the independent sampler.
+        device: CUDA device to compute on.
+    """
+
+    def __init__(self, *, seed: int | None = None, independent_sampler=None, n_startup_trials: int = 10,
+                 deterministic_objective: bool = False, constraints_func=None, warn_independent_sampling: bool = True,
+                 device: int = 0) -> None:
+        super().__init__(seed=seed, independent_sampler=independent_sampler, n_startup_trials=n_startup_trials,
+                         deterministic_objective=deterministic_objective, constraints_func=constraints_func,
+                         warn_independent_sampling=warn_independent_sampling)
+        self._device = device
+        self._engines: list = []   # one per GP: the objectives', then the constraints'
+        # study.optimize(n_jobs > 1) samples on several threads, and a trial's fits, conditioning and queries on the
+        # shared engines must not interleave with another trial's
+        self._lock = threading.RLock()
+
+    def close(self) -> None:
+        with self._lock:
+            for engine in self._engines:
+                engine.close()
+            self._engines = []
+
+    def __del__(self) -> None:  # pragma: no cover
+        try:
+            self.close()
+        except Exception:
+            pass
+
+    def _fit_gp(self, k: int, X: np.ndarray, y: np.ndarray, is_categorical: np.ndarray,
+                cache: _DeviceGP | None) -> _DeviceGP:
+        """``gp.fit_kernel_params`` (gp.py:354-409) on engine ``k``, warm-started from ``cache``'s parameters."""
+        while len(self._engines) <= k:
+            self._engines.append(_engine_cls(self._device))
+        engine = self._engines[k]
+        engine.gp_set_data(X, y, is_categorical)
+        params = _fit(engine, X.shape[1], self._log_prior, self._minimum_noise,
+                      None if cache is None else cache._params, self._deterministic)
+        return _DeviceGP(engine, X, y, is_categorical, params)
+
+    def _get_constraints_acqf_args(self, constraint_vals: np.ndarray,
+                                   internal_search_space: gp_search_space.SearchSpace,
+                                   normalized_params: np.ndarray) -> tuple[list[_DeviceGP], list[float]]:
+        # optuna/samplers/_gp/sampler.py:254-292, with the fits on the device
+        standardized_constraint_vals, means, stds = _standardize_values(-constraint_vals)
+        if (
+            self._gprs_cache_list is not None
+            and len(self._gprs_cache_list[0].inverse_squared_lengthscales) != internal_search_space.dim
+        ):
+            self._constraints_gprs_cache_list = None
+
+        is_categorical = internal_search_space.is_categorical
+        constraints_threshold_list = (-means / np.maximum(EPS, stds)).tolist()
+        first = len(self._gprs_cache_list)   # the objectives' engines come first
+        constraints_gprs = []
+        for i, vals in enumerate(standardized_constraint_vals.T):
+            cache = self._constraints_gprs_cache_list[i] if self._constraints_gprs_cache_list is not None else None
+            constraints_gprs.append(self._fit_gp(first + i, normalized_params, vals, is_categorical, cache))
+
+        self._constraints_gprs_cache_list = constraints_gprs
+        return constraints_gprs, constraints_threshold_list
+
+    def _sample_relative_impl(self, study, completed_trials, trials, search_space) -> dict[str, Any]:
+        with self._lock:
+            return self._sample_relative_locked(study, completed_trials, trials, search_space)
+
+    def _sample_relative_locked(self, study, completed_trials, trials, search_space) -> dict[str, Any]:
+        # optuna/samplers/_gp/sampler.py:358-485, with the fits on the device
+        internal_search_space = gp_search_space.SearchSpace(search_space)
+        normalized_params = internal_search_space.get_normalized_params(completed_trials)
+
+        _sign = np.array([-1.0 if d == StudyDirection.MINIMIZE else 1.0 for d in study.directions])
+        standardized_score_vals, _, _ = _standardize_values(
+            _sign * np.array([trial.values for trial in completed_trials])
+        )
+
+        if (
+            self._gprs_cache_list is not None
+            and len(self._gprs_cache_list[0].inverse_squared_lengthscales) != internal_search_space.dim
+        ):
+            self._gprs_cache_list = None
+
+        gprs_list = []
+        n_objectives = standardized_score_vals.shape[-1]
+        is_categorical = internal_search_space.is_categorical
+        for i in range(n_objectives):
+            cache = self._gprs_cache_list[i] if self._gprs_cache_list is not None else None
+            gprs_list.append(self._fit_gp(i, normalized_params, standardized_score_vals[:, i], is_categorical, cache))
+        self._gprs_cache_list = gprs_list
+
+        best_params: np.ndarray | None
+        acqf: acqf_module.BaseAcquisitionFunc
+        if self._constraints_func is None:
+            if n_objectives == 1:
+                acqf = acqf_module.LogEI(
+                    gpr=gprs_list[0],
+                    search_space=internal_search_space,
+                    threshold=standardized_score_vals[:, 0].max(),
+                    normalized_params_of_running_trials=(
+                        self._get_normalized_params_of_running_trials(trials, internal_search_space)
+                    ),
+                )
+                best_params = normalized_params[np.argmax(standardized_score_vals), np.newaxis]
+            else:
+                acqf = acqf_module.LogEHVI(
+                    gpr_list=gprs_list,
+                    search_space=internal_search_space,
+                    Y_train=torch.from_numpy(standardized_score_vals),
+                    n_qmc_samples=128,
+                    qmc_seed=self._rng.rng.randint(1 << 30),
+                )
+                best_params = self._get_best_params_for_multi_objective(normalized_params, standardized_score_vals)
+        else:
+            constraint_vals, is_feasible = _get_constraint_vals_and_feasibility(study, completed_trials)
+            constr_gpr_list, constr_threshold_list = self._get_constraints_acqf_args(
+                constraint_vals, internal_search_space, normalized_params
+            )
+            if n_objectives == 1:
+                y_with_neginf = np.where(is_feasible, standardized_score_vals[:, 0], -np.inf)
+                i_opt = np.argmax(y_with_neginf)
+                best_feasible_y = y_with_neginf[i_opt]
+                acqf = acqf_module.ConstrainedLogEI(
+                    gpr=gprs_list[0],
+                    search_space=internal_search_space,
+                    threshold=best_feasible_y,
+                    constraints_gpr_list=constr_gpr_list,
+                    constraints_threshold_list=constr_threshold_list,
+                )
+                best_params = None if np.isneginf(best_feasible_y) else normalized_params[i_opt, np.newaxis]
+            else:
+                is_all_infeasible = not any(is_feasible)
+                acqf = acqf_module.ConstrainedLogEHVI(
+                    gpr_list=gprs_list,
+                    search_space=internal_search_space,
+                    Y_feasible=(
+                        torch.from_numpy(standardized_score_vals[is_feasible]) if not is_all_infeasible else None
+                    ),
+                    n_qmc_samples=128,
+                    qmc_seed=self._rng.rng.randint(1 << 30),
+                    constraints_gpr_list=constr_gpr_list,
+                    constraints_threshold_list=constr_threshold_list,
+                )
+                best_params = (
+                    self._get_best_params_for_multi_objective(
+                        normalized_params[is_feasible], standardized_score_vals[is_feasible]
+                    )
+                    if not is_all_infeasible
+                    else None
+                )
+
+        normalized_param = self._optimize_acqf(acqf, best_params)
+        return internal_search_space.get_unnormalized_param(normalized_param)
