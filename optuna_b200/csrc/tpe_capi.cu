@@ -188,8 +188,8 @@ struct tpe_ctx {
   int64_t N = 0;
   // MOTPE scratch
   DevBuf mo_list, mo_alive, mo_dom, mo_first, mo_rank, mo_ctr, mo_tie, mo_ntie, mo_lexpos, mo_isdup, mo_sorted,
-      mo_uniq, mo_nuniq, mo_ref, mo_removed, mo_contrib, mo_state, mo_arena, mo_chosen, mo_diag, mo_w, mo_table, mo_sample,
-      mo_surv, mo_nsurv, mo_fv, mo_ps, mo_map, mo_front, mo_head;
+      mo_uniq, mo_nuniq, mo_ref, mo_removed, mo_contrib, mo_bound, mo_state, mo_arena, mo_chosen, mo_diag, mo_w, mo_table,
+      mo_sample, mo_surv, mo_nsurv, mo_fv, mo_ps, mo_map, mo_front, mo_head;
   bool mo_weights_ready = false;
   std::vector<uint8_t> col_missing, col_oor, col_offgrid;   // col_offgrid: a step column holds a value off its grid
   bool history_set = false;
@@ -729,12 +729,8 @@ int mo_select_complete(tpe_ctx* ctx, int64_t n_below, int64_t* taken) {
     ctx->launch_counter += 1;
     bool finite = true;
     for (int j = 0; j < M; ++j) finite = finite && std::isfinite(ref[j]);
-    std::vector<int32_t> chosen;
-    int n_chosen = subset;
-    bool chosen_on_device = false;
-    if (!finite) {
-      for (int i = 0; i < subset; ++i) chosen.push_back(i);  // rank_i_indices[:subset_size] (hssp.py:106-107)
-    } else {
+    const int n_chosen = subset;
+    {
       k_mo_lexrank<<<(n_tie + 127) / 128, 128, 0, st>>>(vals, M, dlist, ctx->mo_tie.as<int32_t>(), n_tie,
                                                          ctx->mo_lexpos.as<int32_t>(), ctx->mo_isdup.as<uint8_t>());
       k_mo_unique<<<1, 1024, 0, st>>>(n_tie, ctx->mo_lexpos.as<int32_t>(), ctx->mo_isdup.as<uint8_t>(),
@@ -743,7 +739,6 @@ int mo_select_complete(tpe_ctx* ctx, int64_t n_below, int64_t* taken) {
       int nu = 0;
       CU(cudaMemcpyAsync(&nu, ctx->mo_nuniq.p, 4, cudaMemcpyDeviceToHost, st));
       CU(cudaStreamSynchronize(st));
-      chosen_on_device = true;
       if (nu <= subset) {
         // every unique vector, then the first duplicates in trial order (hssp.py:162-171)
         CU(cudaMemcpyAsync(ctx->mo_chosen.p, ctx->mo_uniq.p, (size_t)nu * 4, cudaMemcpyDeviceToDevice, st));
@@ -752,6 +747,9 @@ int mo_select_complete(tpe_ctx* ctx, int64_t n_below, int64_t* taken) {
                                              ctx->mo_chosen.as<int32_t>(), nu);
           ctx->launch_counter++;
         }
+      } else if (!finite) {
+        // the first `subset` unique vectors in lexicographic order (hssp.py:106-107 sees np.unique's output)
+        CU(cudaMemcpyAsync(ctx->mo_chosen.p, ctx->mo_uniq.p, (size_t)subset * 4, cudaMemcpyDeviceToDevice, st));
       } else {
         CU(ctx->mo_state.ensure(hssp_bytes(subset, M)));
         CU(cudaMemsetAsync(ctx->mo_state.p, 0, hssp_bytes(subset, M), st));
@@ -772,7 +770,7 @@ int mo_select_complete(tpe_ctx* ctx, int64_t n_below, int64_t* taken) {
           const int cthreads = sstride ? 32 : 64;
           const size_t csmem = sstride ? (size_t)cthreads * sstride * 8 : 0;
           // more than three objectives: one warp per candidate, a private WFG arena per lane (global memory);
-          // falls back to one thread per candidate when that would need more than 2 GB
+          // falls back to one thread per candidate when that would need more than 8 GB
           const size_t nd_lane_stride = hv_lane_doubles(subset, M);
           const size_t nd_warp_stride = hv_warp_scratch_doubles(subset, M) + 32 * nd_lane_stride;
           const bool nd_warp = M > 3 && (size_t)nu * nd_warp_stride * 8 <= ((size_t)8 << 30);
@@ -781,6 +779,7 @@ int mo_select_complete(tpe_ctx* ctx, int64_t n_below, int64_t* taken) {
           if (!nd_warp && M > 3 && (size_t)nu * stride * 8 > ((size_t)32 << 30))
             return fail(ctx, TPE_E_NOMEM, "MOTPE subset selection: %d candidates x %d picks in %d objectives need %zu GB of "
                         "hypervolume scratch", nu, subset, M, ((size_t)nu * stride * 8) >> 30);
+          CU(ctx->mo_bound.ensure((size_t)nu * 16));   // lazy bounds + k_hssp_pick's scratch
           if (nd_warp) CU(ctx->mo_arena.ensure((size_t)nu * nd_warp_stride * 8));
           else if (big3) CU(ctx->mo_arena.ensure((size_t)nu * stride3 * 8));
           else if (!sstride && M != 3) CU(ctx->mo_arena.ensure((size_t)nu * stride * 8));
@@ -792,21 +791,22 @@ int mo_select_complete(tpe_ctx* ctx, int64_t n_below, int64_t* taken) {
                                                             ctx->mo_uniq.as<int32_t>(), nu,
                                                             ctx->mo_removed.as<uint8_t>(), ctx->mo_ref.as<double>(),
                                                             ctx->mo_state.as<HsspState>(), ctx->mo_contrib.as<double>(),
-                                                            ctx->mo_arena.as<double>(), stride3);
+                                                            ctx->mo_bound.as<double>(), ctx->mo_arena.as<double>(), stride3);
             } else if (nd_warp) {
               k_hssp_contrib_nd<<<(nu + 3) / 4, 128, 0, st>>>(
                   vals, M, dlist, ctx->mo_tie.as<int32_t>(), ctx->mo_uniq.as<int32_t>(), nu,
                   ctx->mo_removed.as<uint8_t>(), ctx->mo_ref.as<double>(), ctx->mo_state.as<HsspState>(),
-                  ctx->mo_contrib.as<double>(), ctx->mo_arena.as<double>(), nd_warp_stride, nd_lane_stride);
+                  ctx->mo_contrib.as<double>(), ctx->mo_bound.as<double>(), ctx->mo_arena.as<double>(), nd_warp_stride,
+                  nd_lane_stride);
             } else {
               k_hssp_contrib<<<(nu + cthreads - 1) / cthreads, cthreads, csmem, st>>>(
                   vals, M, dlist, ctx->mo_tie.as<int32_t>(), ctx->mo_uniq.as<int32_t>(), nu,
                   ctx->mo_removed.as<uint8_t>(), ctx->mo_ref.as<double>(), ctx->mo_state.as<HsspState>(),
-                  ctx->mo_contrib.as<double>(), ctx->mo_arena.as<double>(), stride, sstride);
+                  ctx->mo_contrib.as<double>(), ctx->mo_bound.as<double>(), ctx->mo_arena.as<double>(), stride, sstride);
             }
             k_hssp_pick<<<1, 256, 0, st>>>(vals, M, dlist, ctx->mo_tie.as<int32_t>(), ctx->mo_uniq.as<int32_t>(), nu,
                                            ctx->mo_removed.as<uint8_t>(), ctx->mo_contrib.as<double>(),
-                                           ctx->mo_state.as<HsspState>());
+                                           ctx->mo_bound.as<double>(), ctx->mo_state.as<HsspState>());
             ctx->launch_counter += 2;
           }
         }
@@ -814,8 +814,6 @@ int mo_select_complete(tpe_ctx* ctx, int64_t n_below, int64_t* taken) {
                            (size_t)subset * 4, cudaMemcpyDeviceToDevice, st));
       }
     }
-    if (!chosen_on_device)
-      CU(cudaMemcpyAsync(ctx->mo_chosen.p, chosen.data(), (size_t)n_chosen * 4, cudaMemcpyHostToDevice, st));
     k_mo_mark<<<(n_chosen + 127) / 128, 128, 0, st>>>(dlist, ctx->mo_tie.as<int32_t>(), ctx->mo_chosen.as<int32_t>(),
                                                       n_chosen, ctx->member.as<uint8_t>());
     ctx->launch_counter++;
@@ -2223,7 +2221,7 @@ void tpe_ctx_destroy(tpe_ctx* ctx) {
                     &ctx->mo_first, &ctx->mo_rank, &ctx->mo_ctr, &ctx->mo_tie, &ctx->mo_ntie, &ctx->mo_lexpos,
                     &ctx->mo_isdup, &ctx->mo_sorted, &ctx->mo_uniq, &ctx->mo_nuniq, &ctx->mo_ref, &ctx->mo_removed, &ctx->mo_table,
                     &ctx->mo_sample, &ctx->mo_surv, &ctx->mo_nsurv, &ctx->mo_fv, &ctx->mo_ps, &ctx->mo_map, &ctx->mo_front, &ctx->mo_head,
-                    &ctx->mo_contrib, &ctx->mo_state, &ctx->mo_arena, &ctx->mo_chosen, &ctx->mo_diag, &ctx->mo_w, &ctx->cols, &ctx->row_ok, &ctx->member,
+                    &ctx->mo_contrib, &ctx->mo_bound, &ctx->mo_state, &ctx->mo_arena, &ctx->mo_chosen, &ctx->mo_diag, &ctx->mo_w, &ctx->cols, &ctx->row_ok, &ctx->member,
                     &ctx->counts, &ctx->split_work, &ctx->below_all, &ctx->kpart, &ctx->mixcols, &ctx->ub_arena, &ctx->ub_ord_a, &ctx->ub_ord_b, &ctx->ub_wstage, &ctx->uxs, &ctx->ucidx, &ctx->uni_prev_rows, &ctx->uni_mode, &ctx->uni_work, &ctx->sort_val, &ctx->sort_idx, &ctx->sort_work, &ctx->U, &ctx->S,
                     &ctx->xT, &ctx->x64s, &ctx->x32s, &ctx->e32s, &ctx->gmax, &ctx->lse_gmax, &ctx->mt_state, &ctx->U2, &ctx->mt_spec, &ctx->mt_jump, &ctx->mt_tmp, &ctx->oob, &ctx->logl, &ctx->logg, &ctx->out_x, &ctx->out_acq, &ctx->out_best})
     b->release();

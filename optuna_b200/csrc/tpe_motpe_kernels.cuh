@@ -273,6 +273,23 @@ __host__ __device__ inline size_t hssp_bytes(int cap, int M) {
   return sizeof(HsspState) + (size_t)cap * M * 8 + (size_t)cap * 4 + 8;
 }
 
+// The reference's lazily updated upper bound of a candidate's contribution (hssp.py:68-77), one per unique
+// candidate, kept across rounds: the first round's bound is the candidate's own box incl; later rounds cap the
+// previous value (what the last scan left: exact, bound or inf) by the contribution to the newest pick alone,
+// incl - |box(max(me, last pick))|; every bound is inf once the selected hypervolume is (hssp.py:68-70).
+// np.minimum propagates NaN (inf - inf when both boxes are infinite).
+__device__ __forceinline__ double hssp_bound(const double* me, int M, const double* ref, const HsspState* st,
+                                             double incl, double prev) {
+  const int t = st->n_sel;
+  if (t == 0) return incl;
+  if (isinf(st->hv)) return INFINITY;
+  const double* last = hssp_sel(st) + (size_t)(t - 1) * M;
+  double cap = 1.0;
+  for (int j = 0; j < M; ++j) cap = TPE_MUL(cap, TPE_SUB(ref[j], me[j] > last[j] ? me[j] : last[j]));
+  const double b = TPE_SUB(incl, cap);
+  return (prev != prev || b != b) ? NAN : (b < prev ? b : prev);
+}
+
 // Warp-cooperative exact 3-D hypervolume of n <= kMoMaxSet + 1 mutually non-dominated points
 // (the assume_pareto branch of hypervolume()), bit-identical to it: the two stable insertion sorts
 // become ranks by counting, every row's inner sum is evaluated by one lane exactly as hv_3d does,
@@ -333,8 +350,8 @@ __global__ void __launch_bounds__(128)
 k_hssp_contrib3(const double* __restrict__ vals, const int64_t* __restrict__ list,
                 const int32_t* __restrict__ tie_pos, const int32_t* __restrict__ uniq, int nu,
                 const uint8_t* __restrict__ removed, const double* __restrict__ ref,
-                const HsspState* __restrict__ st, double* __restrict__ contrib, double* __restrict__ arena,
-                size_t arena_stride) {
+                const HsspState* __restrict__ st, double* __restrict__ contrib, double* __restrict__ bound,
+                double* __restrict__ arena, size_t arena_stride) {
   __shared__ double s_scr[4][kHv3Scratch];
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int u = blockIdx.x * 4 + w;
@@ -346,6 +363,7 @@ k_hssp_contrib3(const double* __restrict__ vals, const int64_t* __restrict__ lis
   const double* me = vals + list[tie_pos[uniq[u]]] * 3;
   double incl = 1.0;
   for (int j = 0; j < 3; ++j) incl = TPE_MUL(incl, TPE_SUB(ref[j], me[j]));
+  if (lane == 0) { bound[u] = hssp_bound(me, 3, ref, st, incl, bound[u]); bound[nu + u] = incl; }
   const int t = st->n_sel;
   if (t == 0 || isinf(incl)) {
     if (lane == 0) contrib[u] = incl;
@@ -494,8 +512,8 @@ __global__ void __launch_bounds__(128)
 k_hssp_contrib_nd(const double* __restrict__ vals, int M, const int64_t* __restrict__ list,
                   const int32_t* __restrict__ tie_pos, const int32_t* __restrict__ uniq, int nu,
                   const uint8_t* __restrict__ removed, const double* __restrict__ ref,
-                  const HsspState* __restrict__ st, double* __restrict__ contrib, double* __restrict__ arena,
-                  size_t warp_stride, size_t lane_stride) {
+                  const HsspState* __restrict__ st, double* __restrict__ contrib, double* __restrict__ bound,
+                  double* __restrict__ arena, size_t warp_stride, size_t lane_stride) {
   const int lane = threadIdx.x & 31;
   const int u = blockIdx.x * 4 + (threadIdx.x >> 5);
   if (u >= nu) return;
@@ -506,6 +524,7 @@ k_hssp_contrib_nd(const double* __restrict__ vals, int M, const int64_t* __restr
   const double* me = vals + list[tie_pos[uniq[u]]] * M;
   double incl = 1.0;
   for (int j = 0; j < M; ++j) incl = TPE_MUL(incl, TPE_SUB(ref[j], me[j]));
+  if (lane == 0) { bound[u] = hssp_bound(me, M, ref, st, incl, bound[u]); bound[nu + u] = incl; }
   const int t = st->n_sel;
   if (t == 0 || isinf(incl)) {
     if (lane == 0) contrib[u] = incl;
@@ -529,12 +548,12 @@ k_hssp_contrib_nd(const double* __restrict__ vals, int M, const int64_t* __restr
   if (lane == 0) contrib[u] = TPE_SUB(incl, hv);
 }
 
-// Exact contribution of every remaining unique candidate given the selected set
-// (hssp.py:45-97 evaluated without the lazy skipping, which cannot change the argmax).
+// Exact contribution of every remaining unique candidate given the selected set (hssp.py:87-95) and its lazy
+// bound (hssp_bound), and its own box incl in bound[nu + u]; k_hssp_pick decides which the reference's scan keeps.
 __global__ void k_hssp_contrib(const double* __restrict__ vals, int M, const int64_t* __restrict__ list,
                                const int32_t* __restrict__ tie_pos, const int32_t* __restrict__ uniq, int nu,
                                const uint8_t* __restrict__ removed, const double* __restrict__ ref,
-                               const HsspState* __restrict__ st, double* __restrict__ contrib,
+                               const HsspState* __restrict__ st, double* __restrict__ contrib, double* __restrict__ bound,
                                double* __restrict__ arena, size_t arena_stride, int smem_stride) {
   // smem_stride != 0 (M <= 3, where the scratch is a few hundred doubles per thread): the scratch
   // lives in shared memory instead of the global arena
@@ -548,6 +567,8 @@ __global__ void k_hssp_contrib(const double* __restrict__ vals, int M, const int
   const double* me = vals + list[tie_pos[uniq[u]]] * M;
   double incl = 1.0;
   for (int j = 0; j < M; ++j) incl = TPE_MUL(incl, TPE_SUB(ref[j], me[j]));
+  bound[u] = hssp_bound(me, M, ref, st, incl, bound[u]);
+  bound[nu + u] = incl;
   const int t = st->n_sel;
   if (t == 0 || isinf(incl)) {
     contrib[u] = incl;
@@ -576,22 +597,9 @@ __global__ void k_hssp_contrib(const double* __restrict__ vals, int M, const int
     contrib[u] = TPE_SUB(incl, hypervolume(pts, t, M, ref, false, rest));
   }
 }
-// first argmax (lexicographic order of the unique list), append to the selected set
-__global__ void __launch_bounds__(256)
-k_hssp_pick(const double* __restrict__ vals, int M, const int64_t* __restrict__ list,
-            const int32_t* __restrict__ tie_pos, const int32_t* __restrict__ uniq, int nu,
-            uint8_t* __restrict__ removed, const double* __restrict__ contrib, HsspState* __restrict__ st) {
-  __shared__ double s_val[256];
-  __shared__ int s_idx[256];
-  double best = -INFINITY;
-  int bi = -1;
-  bool bnan = false;
-  for (int u = threadIdx.x; u < nu; u += 256) {
-    if (removed[u]) continue;
-    const double c = contrib[u];
-    const bool cn = c != c;
-    if (bi < 0 || (!bnan && (cn || c > best))) { best = c; bi = u; bnan = cn; }
-  }
+// First argmax over a 256-thread block of one (value, index) candidate per thread (index < 0: none): np.argmax
+// semantics, the first NaN wins, ties go to the smaller index.  Result in s_val[0] / s_idx[0].
+__device__ void block_first_argmax256(double best, int bi, double* s_val, int* s_idx) {
   s_val[threadIdx.x] = best;
   s_idx[threadIdx.x] = bi;
   __syncthreads();
@@ -613,9 +621,101 @@ k_hssp_pick(const double* __restrict__ vals, int M, const int64_t* __restrict__ 
     }
     __syncthreads();
   }
+}
+__device__ __forceinline__ void argmax_step(double c, int u, double& best, int& bi, bool& bnan) {
+  const bool cn = c != c;
+  if (bi < 0 || (!bnan && (cn || c > best))) { best = c; bi = u; bnan = cn; }
+}
+
+constexpr int kPickStage = 1024;   // candidates whose bounds and exact values k_hssp_pick stages in shared memory
+
+// The value the reference's scan leaves for remaining candidate u (see k_hssp_pick): inf for an infinite own box;
+// its bound b when b < 0 or a candidate visited earlier (larger bound, or equal bound and smaller index) has an
+// exact value above b; else its exact value.  A removed candidate has exact value -inf and never decides.
+// js >= 0: a candidate with the largest exact value ejs and bound bjs, tried first.
+__device__ __forceinline__ double hssp_scan_value(int u, int nu, double incl, const double* B, const double* E, int js,
+                                                  double ejs, double bjs) {
+  if (isinf(incl)) return INFINITY;
+  const double b = B[u];
+  bool keep = !(b >= 0.0);
+  if (!keep && js >= 0 && js != u && (bjs > b || (bjs == b && js < u)) && ejs > b) keep = true;
+  for (int q = 0; q < nu && !keep; ++q) {
+    const double bq = B[q];
+    keep = q != u && (bq > b || (bq == b && q < u)) && E[q] > b;
+  }
+  return keep ? b : E[u];
+}
+
+// One round of the reference's greedy pick (hssp.py:78-97, then :123): the lazy scan over the remaining unique
+// candidates, then the first argmax of what it leaves, appended to the selected set.
+// The scan visits candidates in descending bound order, ties by ascending index (a stable argsort; numpy's is not
+// stable, so where bounds tie the reference's own visiting order is unspecified).  A candidate whose own box is
+// infinite becomes inf; one whose bound is below the best exact value seen so far keeps its bound; any other takes
+// its exact value.  As bounds only fall along the visiting order and the best only rises, a candidate keeps its bound
+// exactly when its bound is < 0 or a candidate visited before it has an exact value above that bound, which every
+// thread decides for its own candidates without a sequential pass.
+//   contrib: exact contributions (k_hssp_contrib*; -inf for removed candidates);
+//   bound: [0, nu) lazy bounds in, the scan's values out; [nu, 2 nu) each candidate's incl in, scratch
+__global__ void __launch_bounds__(256)
+k_hssp_pick(const double* __restrict__ vals, int M, const int64_t* __restrict__ list,
+            const int32_t* __restrict__ tie_pos, const int32_t* __restrict__ uniq, int nu,
+            uint8_t* __restrict__ removed, const double* __restrict__ contrib, double* __restrict__ bound,
+            HsspState* __restrict__ st) {
+  __shared__ double s_val[256];
+  __shared__ int s_idx[256];
+  __shared__ double s_b[kPickStage], s_e[kPickStage];
+  double* scan = bound + nu;
+  const int t = st->n_sel;
+  double best = -INFINITY;
+  int bi = -1;
+  bool bnan = false;
+  if (t == 0 || isinf(st->hv)) {   // first round: bound = exact = incl; inf hypervolume: every value is inf
+    for (int u = threadIdx.x; u < nu; u += 256)
+      if (!removed[u]) argmax_step(bound[u], u, best, bi, bnan);
+  } else if (nu <= kPickStage) {
+    // every thread keeps the values of its (at most four) candidates in registers
+    double mine[kPickStage / 256], incl[kPickStage / 256];
+#pragma unroll
+    for (int k = 0; k < kPickStage / 256; ++k) {
+      const int u = threadIdx.x + k * 256;
+      if (u < nu) { s_b[u] = bound[u]; s_e[u] = contrib[u]; incl[k] = scan[u]; }
+    }
+    __syncthreads();
+#pragma unroll
+    for (int k = 0; k < kPickStage / 256; ++k) {
+      const int u = threadIdx.x + k * 256;
+      if (u < nu) mine[k] = hssp_scan_value(u, nu, incl[k], s_b, s_e, -1, 0.0, 0.0);
+    }
+#pragma unroll
+    for (int k = 0; k < kPickStage / 256; ++k) {
+      const int u = threadIdx.x + k * 256;
+      if (u < nu && !removed[u]) {
+        bound[u] = mine[k];
+        argmax_step(mine[k], u, best, bi, bnan);
+      }
+    }
+  } else {
+    // the best exact value: usually visited early, it decides most candidates at once
+    for (int u = threadIdx.x; u < nu; u += 256)
+      if (!removed[u]) argmax_step(contrib[u], u, best, bi, bnan);
+    block_first_argmax256(best, bi, s_val, s_idx);
+    const int js = s_idx[0];
+    const double ejs = s_val[0], bjs = bound[js];
+    for (int u = threadIdx.x; u < nu; u += 256)
+      if (!removed[u]) scan[u] = hssp_scan_value(u, nu, scan[u], bound, contrib, js, ejs, bjs);
+    __syncthreads();
+    best = -INFINITY;
+    bi = -1;
+    bnan = false;
+    for (int u = threadIdx.x; u < nu; u += 256)
+      if (!removed[u]) {
+        bound[u] = scan[u];
+        argmax_step(scan[u], u, best, bi, bnan);
+      }
+  }
+  block_first_argmax256(best, bi, s_val, s_idx);
   if (threadIdx.x == 0) {
     const int u = s_idx[0];
-    const int t = st->n_sel;
     st->hv = TPE_ADD(st->hv, s_val[0]);
     hssp_pick(st, M)[t] = uniq[u];
     const double* me = vals + list[tie_pos[uniq[u]]] * M;
