@@ -41,7 +41,8 @@ extern "C" {
 /* 10: + tpe_gp_set_data, tpe_gp_loss, tpe_gp_posterior, TPE_E_NOTPD */
 /* 11: + tpe_gp_loss_fixed_noise, tpe_gp_posterior_moments */
 /* 12: + tpe_gp_condition, tpe_gp_query */
-#define TPE_ABI_VERSION 12
+/* 13: + tpe_ehvi_set, tpe_ehvi */
+#define TPE_ABI_VERSION 13
 
 enum {
   TPE_OK = 0,
@@ -334,6 +335,22 @@ int tpe_gp_posterior_moments(tpe_ctx* ctx, const double* params, const double* X
                              double* mean, double* var, double* cov);
 int tpe_gp_condition(tpe_ctx* ctx, const double* params);
 int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double* var, double* dmean, double* dvar);
+/* Log expected hypervolume improvement of GPSampler's multi-objective acquisition (LogEHVI, optuna/_gp/acqf.py:245-300,
+ * with logehvi :45-62), fp64.  Kept apart from the history, the suggestion state and the GP state.
+ * tpe_ehvi_set replaces the state LogEHVI.__init__ builds (acqf.py:245-280): lower [B, M] the lower bounds of the
+ * non-dominated boxes, intervals [B, M] their widths already clamped at 1e-12, samples [S, M] the fixed QMC samples
+ * (standard normal).  2 <= M <= 24 (a product of M factors of at least 1e-12 stays a normal double), 1 <= S <= 1024,
+ * B >= 1, no NaN; infinities are allowed and follow IEEE arithmetic as torch does (an interval is often +inf, a sample
+ * can be -inf).  TPE_E_INVALID naming the violated condition.
+ * tpe_ehvi replaces LogEHVI.eval_acqf after the posteriors (acqf.py:282-300) and its autograd backward: at Q rows of
+ * posterior means mean [Q, M] and standard deviations sd [Q, M], value [Q] = log(1/S sum_{s,b} prod_j
+ * min(max(mean_j + sd_j z_sj - lower_bj, 1e-12), intervals_bj)), the reference's logsumexp of sum_j log; with dmean and
+ * dsd non-NULL (both or neither) also its gradients [Q, M] in mean and sd, through torch's inclusive clamp mask.  A
+ * row's value is the same bits whatever Q, the row's position and the gradient request, and repeated calls return the
+ * same bits.  TPE_E_STATE before tpe_ehvi_set. */
+int tpe_ehvi_set(tpe_ctx* ctx, const double* lower, const double* intervals, int64_t B, const double* samples,
+                 int32_t S, int32_t M);
+int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, double* value, double* dmean, double* dsd);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

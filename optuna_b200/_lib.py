@@ -81,6 +81,8 @@ SYMBOLS = {
     "tpe_gp_posterior_moments": (C.c_int, [_P, _P, _P, C.c_int64, C.c_int32, _P, _P, _P]),
     "tpe_gp_condition": (C.c_int, [_P, _P]),
     "tpe_gp_query": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P, _P]),
+    "tpe_ehvi_set": (C.c_int, [_P, _P, _P, C.c_int64, _P, C.c_int32, C.c_int32]),
+    "tpe_ehvi": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, _P]),
     "tpe_get_candidates": (C.c_int, [_P, _P, _P, _P]),
     "tpe_logpdf": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P]),
     "tpe_last_timing": (C.c_int, [_P, _P, _P]),
@@ -91,7 +93,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 12  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 13  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

@@ -23,6 +23,7 @@
 #include "tpe_pareto.cuh"
 #include "tpe_fanova.cuh"
 #include "tpe_gp.cuh"
+#include "tpe_ehvi.cuh"
 #include "tpe_uni.cuh"
 #include "tpe_mixed.cuh"
 #include "tpe_tcscreen.cuh"
@@ -132,6 +133,19 @@ struct GpState {
                     (void*)cat, (void*)fail})
       if (p) cudaFree(p);
     *this = GpState();
+  }
+};
+
+// log-EHVI of GPSampler's multi-objective acquisition (tpe_ehvi_*, tpe_ehvi.cuh): the box decomposition and the QMC
+// samples of tpe_ehvi_set, and the per-call buffers of tpe_ehvi
+struct EhviState {
+  int64_t B = 0;
+  int32_t S = 0, M = 0;
+  DevBuf lbI, Z, mean, sd, part, value, dmean, dsd;
+  bool ready = false;
+  void release() {
+    for (DevBuf* b : {&lbI, &Z, &mean, &sd, &part, &value, &dmean, &dsd}) b->release();
+    *this = EhviState();
   }
 };
 
@@ -269,6 +283,7 @@ struct tpe_ctx {
   int32_t uni_ord_col = -1;
   int64_t uni_ord_K = -1;
   GpState gp;
+  EhviState ehvi;
 };
 
 namespace {
@@ -2228,6 +2243,7 @@ void tpe_ctx_destroy(tpe_ctx* ctx) {
   ctx->est[0].release();
   ctx->est[1].release();
   ctx->gp.release();
+  ctx->ehvi.release();
   if (ctx->res_host) cudaFreeHost(ctx->res_host);
   if (ctx->mt_host) cudaFreeHost(ctx->mt_host);
   if (ctx->up_host) cudaFreeHost(ctx->up_host);
@@ -3896,6 +3912,113 @@ int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(mean, g.ucb, m * 8, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(var, g.lcb, m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
+// ---- log-EHVI of GPSampler's multi-objective acquisition (tpe_ehvi.cuh) ----------------------------------------------
+static constexpr int64_t kEhviPartDoubles = (int64_t)1 << 23;   // partial sums of one launch at most (64 MB)
+
+// the chunk kernel for M objectives: register arrays sized for the next of 4, 8, 12, 24 (a 16 spills with gradients)
+typedef void (*EhviChunkFn)(const double*, int64_t, const double*, int, int, const double*, const double*, double*);
+static EhviChunkFn ehvi_chunk_kernel(int M, bool grad) {
+  if (M <= 4) return grad ? ehvi::k_ehvi_chunk<4, true> : ehvi::k_ehvi_chunk<4, false>;
+  if (M <= 8) return grad ? ehvi::k_ehvi_chunk<8, true> : ehvi::k_ehvi_chunk<8, false>;
+  if (M <= 12) return grad ? ehvi::k_ehvi_chunk<12, true> : ehvi::k_ehvi_chunk<12, false>;
+  return grad ? ehvi::k_ehvi_chunk<24, true> : ehvi::k_ehvi_chunk<24, false>;
+}
+
+// replaces LogEHVI.__init__'s state (optuna/_gp/acqf.py:245-280): the non-dominated boxes and the fixed QMC samples
+int tpe_ehvi_set(tpe_ctx* ctx, const double* lower, const double* intervals, int64_t B, const double* samples,
+                 int32_t S, int32_t M) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  EhviState& e = ctx->ehvi;
+  e.ready = false;
+  if (M < 2 || M > ehvi::MAX_M) return fail(ctx, TPE_E_INVALID, "EHVI needs 2 <= M <= %d objectives, got %d", ehvi::MAX_M, M);
+  if (S < 1 || S > ehvi::MAX_S) return fail(ctx, TPE_E_INVALID, "EHVI needs 1 <= S <= %d samples, got %d", ehvi::MAX_S, S);
+  if (B < 1 || B > ((int64_t)1 << 31)) return fail(ctx, TPE_E_INVALID, "EHVI needs 1 <= B <= 2^31 boxes, got %lld", (long long)B);
+  if (!lower || !intervals || !samples) return fail(ctx, TPE_E_INVALID, "bad EHVI arguments");
+  std::vector<double> lbI((size_t)B * M * 2);
+  for (int64_t i = 0; i < B * M; ++i) {
+    if (std::isnan(lower[i])) return fail(ctx, TPE_E_INVALID, "EHVI box lower bounds hold a NaN");
+    if (std::isnan(intervals[i])) return fail(ctx, TPE_E_INVALID, "EHVI box intervals hold a NaN");
+    lbI[2 * i] = lower[i];
+    lbI[2 * i + 1] = intervals[i];
+  }
+  for (int64_t i = 0; i < (int64_t)S * M; ++i)
+    if (std::isnan(samples[i])) return fail(ctx, TPE_E_INVALID, "EHVI samples hold a NaN");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  cudaStream_t st = ctx->stream;
+  CU(e.lbI.ensure(lbI.size() * 8));
+  CU(e.Z.ensure((size_t)S * M * 8));
+  CU(cudaMemcpyAsync(e.lbI.p, lbI.data(), lbI.size() * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(e.Z.p, samples, (size_t)S * M * 8, cudaMemcpyHostToDevice, st));
+  for (bool grad : {false, true}) {
+    const size_t smem = ehvi::smem_bytes(M, grad);
+    if (smem > 48 * 1024)
+      CU(cudaFuncSetAttribute(ehvi_chunk_kernel(M, grad), cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  }
+  CU(cudaStreamSynchronize(st));   // the host copy of the bounds goes out of scope
+  e.B = B;
+  e.S = S;
+  e.M = M;
+  e.ready = true;
+  return TPE_OK;
+}
+
+// replaces LogEHVI.eval_acqf after the posteriors (acqf.py:282-300, with logehvi :45-62) and its autograd backward in
+// the posterior mean and standard deviation
+int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, double* value, double* dmean,
+             double* dsd) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  EhviState& e = ctx->ehvi;
+  if (!e.ready) return fail(ctx, TPE_E_STATE, "no EHVI boxes and samples (tpe_ehvi_set)");
+  if (!mean || !sd || !value || Q < 1 || (dmean == nullptr) != (dsd == nullptr))
+    return fail(ctx, TPE_E_INVALID, "bad EHVI arguments");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  const bool grad = dmean != nullptr;
+  const int M = e.M, K = grad ? 1 + 2 * M : 1;
+  const int64_t nchunks = (e.B + ehvi::CHUNK - 1) / ehvi::CHUNK;
+  // rows per launch: the partial sums stay under kEhviPartDoubles and the grid's y extent under 65 535
+  const int64_t slab = std::max<int64_t>(1, std::min<int64_t>({Q, kEhviPartDoubles / (nchunks * K), 65535}));
+  cudaStream_t st = ctx->stream;
+  CU(e.mean.ensure((size_t)Q * M * 8));
+  CU(e.sd.ensure((size_t)Q * M * 8));
+  CU(e.value.ensure((size_t)Q * 8));
+  CU(e.part.ensure((size_t)slab * nchunks * K * 8));
+  if (grad) {
+    CU(e.dmean.ensure((size_t)Q * M * 8));
+    CU(e.dsd.ensure((size_t)Q * M * 8));
+  }
+  CU(cudaMemcpyAsync(e.mean.p, mean, (size_t)Q * M * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(e.sd.p, sd, (size_t)Q * M * 8, cudaMemcpyHostToDevice, st));
+  const size_t smem = ehvi::smem_bytes(M, grad);
+  const double log_s = std::log((double)e.S);
+  for (int64_t r0 = 0; r0 < Q; r0 += slab) {
+    const int64_t rows = std::min(slab, Q - r0);
+    const dim3 grid((unsigned)nchunks, (unsigned)rows);
+    const double* m0 = e.mean.as<double>() + r0 * M;
+    const double* s0 = e.sd.as<double>() + r0 * M;
+    const unsigned fb = (unsigned)((rows + 127) / 128);
+    ehvi_chunk_kernel(M, grad)<<<grid, ehvi::THREADS, smem, st>>>(e.lbI.as<double>(), e.B, e.Z.as<double>(), e.S, M,
+                                                                   m0, s0, e.part.as<double>());
+    if (grad) {
+      ehvi::k_ehvi_finish<true><<<fb, 128, 0, st>>>(e.part.as<double>(), rows, (int)nchunks, M, log_s,
+                                                    e.value.as<double>() + r0, e.dmean.as<double>() + r0 * M,
+                                                    e.dsd.as<double>() + r0 * M);
+    } else {
+      ehvi::k_ehvi_finish<false><<<fb, 128, 0, st>>>(e.part.as<double>(), rows, (int)nchunks, M, log_s,
+                                                     e.value.as<double>() + r0, nullptr, nullptr);
+    }
+  }
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(value, e.value.p, (size_t)Q * 8, cudaMemcpyDeviceToHost, st));
+  if (grad) {
+    CU(cudaMemcpyAsync(dmean, e.dmean.p, (size_t)Q * M * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(dsd, e.dsd.p, (size_t)Q * M * 8, cudaMemcpyDeviceToHost, st));
+  }
   CU(cudaStreamSynchronize(st));
   return TPE_OK;
 }

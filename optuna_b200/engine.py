@@ -61,6 +61,7 @@ class TPEEngine:
         self._specs: list[ParamSpec] = []
         self._cols: list[int] = []
         self._gp_P = 0
+        self._ehvi_M = 0
 
     # -- lifecycle -----------------------------------------------------------------------------
     def close(self) -> None:
@@ -503,6 +504,32 @@ class TPEEngine:
         self._check(self._lib.tpe_gp_query(self._h, _ptr(xq), xq.shape[0], _ptr(mean), _ptr(var), _ptr(dmean),
                                            _ptr(dvar)))
         return (mean, var, dmean, dvar) if grad else (mean, var)
+
+    def ehvi_set(self, lower, intervals, samples) -> None:
+        """The non-dominated boxes and fixed QMC samples of a log-EHVI acquisition (tpe_ehvi_set): ``lower`` and
+        ``intervals`` [B, M] (intervals already clamped at 1e-12), ``samples`` [S, M].  2 <= M <= 24, 1 <= S <= 1024,
+        no NaN (infinities are allowed).  Leaves the history, suggestion and GP state of this engine unchanged."""
+        lb, iv, z = _f64(lower), _f64(intervals), _f64(samples)
+        if lb.ndim != 2 or iv.shape != lb.shape or z.ndim != 2 or z.shape[1] != lb.shape[1]:
+            raise ValueError(f"EHVI inputs must be lower [B, M], intervals [B, M], samples [S, M]; got {lb.shape}, "
+                             f"{iv.shape}, {z.shape}")
+        self._ehvi_M = 0   # a failed call leaves no EHVI state in the context either
+        self._check(self._lib.tpe_ehvi_set(self._h, _ptr(lb), _ptr(iv), lb.shape[0], _ptr(z), z.shape[0], z.shape[1]))
+        self._ehvi_M = lb.shape[1]
+
+    def ehvi(self, mean, sd, grad: bool = False):
+        """log-EHVI at the rows of ``mean`` and ``sd`` [Q, M], the posterior means and standard deviations of the M
+        objectives, against the boxes and samples of ``ehvi_set`` (tpe_ehvi): ``value`` [Q] and with ``grad`` also
+        ``(dmean, dsd)`` [Q, M], its gradients.  The values are the same bits with and without ``grad``."""
+        m, s = _f64(mean), _f64(sd)
+        M = self._ehvi_M
+        if m.ndim != 2 or s.shape != m.shape or (M and m.shape[1] != M):
+            raise ValueError(f"mean and sd must be [Q, {M}], got shapes {m.shape}, {s.shape}")
+        value = np.empty(m.shape[0])
+        dmean = np.empty(m.shape) if grad else None
+        dsd = np.empty(m.shape) if grad else None
+        self._check(self._lib.tpe_ehvi(self._h, _ptr(m), _ptr(s), m.shape[0], _ptr(value), _ptr(dmean), _ptr(dsd)))
+        return (value, dmean, dsd) if grad else value
 
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:

@@ -8,10 +8,16 @@
   n x n factor plus torch autograd for the gradient in x.
 
 This sampler subclasses optuna's and keeps every host step: the standardisation, the cache handling, the choice of
-starting points, the random stream, optuna's acquisition functions and ``optimize_acqf_mixed``.  Only the GPs move to
-the device.  Each GP is fitted by the terminator's device fit (``terminator._fit``: the loss and its gradient on the
+starting points, the random stream, optuna's acquisition functions and ``optimize_acqf_mixed``.  The GPs move to the
+device.  Each GP is fitted by the terminator's device fit (``terminator._fit``: the loss and its gradient on the
 device, scipy's L-BFGS-B and the prior on the host), factorised once, and queried with its posterior and the
 posterior's gradient in x against that factor (``TPEEngine.gp_condition`` / ``gp_query``).
+
+With two or more objectives the log-EHVI of ``LogEHVI`` (acqf.py:45-62, 245-300), and of ``ConstrainedLogEHVI``'s
+objective part, also runs on the device (``TPEEngine.ehvi_set`` / ``ehvi``): optuna builds a (points, 128 samples,
+boxes, objectives) fp64 tensor per evaluation, which at four objectives and a thousand trials is tens of GB.  optuna
+still computes the box decomposition, the QMC samples and the constraints' ``LogPI`` terms on the host; the other
+acquisition functions run unchanged over the device GPs.  Beyond 24 objectives optuna's host ``LogEHVI`` is kept.
 
 One difference: the device holds two n x n fp64 matrices per GP, and ``sample_relative`` raises ``ValueError``
 naming the need when the device lacks that memory.
@@ -34,6 +40,16 @@ from .terminator import _fit
 
 # the engine class that answers the computation (tests substitute a host implementation)
 _engine_cls = TPEEngine
+# objectives the device log-EHVI takes at most (tpe_ehvi_set); beyond, optuna's host LogEHVI runs
+_EHVI_MAX_OBJECTIVES = 24
+
+
+def _answers_ehvi(engine_cls) -> bool:
+    """Whether ``engine_cls`` answers the log-EHVI calls (``ehvi_set`` / ``ehvi``) as well as the GP calls.
+    ``TPEEngine`` always does: its library refuses to load without the EHVI entry points, so on the device a missing
+    kernel is an error.  A substitute engine that restates only the GP calls (a host implementation of them) leaves the
+    acquisition to optuna's host ``LogEHVI``, as before the device log-EHVI existed."""
+    return callable(getattr(engine_cls, "ehvi_set", None)) and callable(getattr(engine_cls, "ehvi", None))
 
 
 def _condition(engine, params: np.ndarray) -> None:
@@ -95,6 +111,52 @@ class _DeviceGP:
         return _Posterior.apply(x, self)
 
 
+class _EHVI(torch.autograd.Function):
+    """``logehvi`` of the stacked posteriors (acqf.py:45-62, 282-300) from one device call; the backward is
+    ``g dvalue/dmean`` and ``g dvalue/dsd`` with the gradients that call returned."""
+
+    @staticmethod
+    def forward(ctx: Any, mean: torch.Tensor, sd: torch.Tensor, engine) -> torch.Tensor:
+        want_grad = ctx.needs_input_grad[0] or ctx.needs_input_grad[1]
+        M = mean.shape[-1]
+        m = mean.detach().cpu().numpy().reshape(-1, M)
+        s = sd.detach().cpu().numpy().reshape(-1, M)
+        out = engine.ehvi(m, s, grad=want_grad)
+        if not want_grad:
+            return torch.from_numpy(out).reshape(mean.shape[:-1])
+        ctx.save_for_backward(torch.from_numpy(out[1]).reshape(mean.shape), torch.from_numpy(out[2]).reshape(sd.shape))
+        return torch.from_numpy(out[0]).reshape(mean.shape[:-1])
+
+    @staticmethod
+    def backward(ctx: Any, g: torch.Tensor) -> tuple[torch.Tensor, torch.Tensor, None]:
+        dmean, dsd = ctx.saved_tensors
+        return g[..., None] * dmean, g[..., None] * dsd, None
+
+
+class _DeviceLogEHVI(acqf_module.BaseAcquisitionFunc):
+    """optuna's ``LogEHVI`` (acqf.py:245-300) with its ``logehvi`` on the device.  It takes an already-built host
+    ``LogEHVI``, so the box decomposition and the QMC samples are the reference's bits, uploads them to ``engine``
+    once, and keeps that object's GPs, stabilising noise, ``length_scales`` and ``search_space``.  ``eval_acqf``
+    forms each objective's standard deviation as the reference does and evaluates log-EHVI and its gradient in one
+    device call."""
+
+    def __init__(self, host: acqf_module.LogEHVI, engine) -> None:
+        self._gpr_list = host._gpr_list
+        self._stabilizing_noise = host._stabilizing_noise
+        self._engine = engine
+        engine.ehvi_set(host._non_dominated_box_lower_bounds.numpy(), host._non_dominated_box_intervals.numpy(),
+                        host._fixed_samples.numpy())
+        super().__init__(host.length_scales, host.search_space)
+
+    def eval_acqf(self, x: torch.Tensor) -> torch.Tensor:
+        means, sds = [], []
+        for gpr in self._gpr_list:
+            mean, var = gpr.posterior(x)
+            means.append(mean)
+            sds.append(torch.sqrt(var + self._stabilizing_noise))
+        return _EHVI.apply(torch.stack(means, dim=-1), torch.stack(sds, dim=-1), self._engine)
+
+
 class GPSampler(_OptunaGPSampler):
     """Gaussian-process Bayesian-optimisation sampler whose Gaussian processes are fitted and queried on the GPU.
 
@@ -103,6 +165,10 @@ class GPSampler(_OptunaGPSampler):
     of the device's fp64 sums.  Its engines (one per objective and per constraint) are kept across trials; ``close``
     frees them.  Under ``study.optimize(n_jobs > 1)`` the relative sampling of concurrent trials runs one at a time,
     since the trials share those engines.
+
+    With 2 to 24 objectives the log-EHVI acquisition (with constraints, its hypervolume part) is also evaluated on
+    the device, by one more engine kept across trials; optuna's other acquisition functions run unchanged over the
+    device GPs.
 
     The device holds two n x n fp64 matrices per GP, n being the number of complete trials (plus the running ones in a
     single-objective study without constraints).  When it lacks that memory, ``sample_relative`` raises
@@ -127,6 +193,7 @@ class GPSampler(_OptunaGPSampler):
                          warn_independent_sampling=warn_independent_sampling)
         self._device = device
         self._engines: list = []   # one per GP: the objectives', then the constraints'
+        self._ehvi_engine = None   # the log-EHVI acquisition's, created on the first multi-objective ask
         # study.optimize(n_jobs > 1) samples on several threads, and a trial's fits, conditioning and queries on the
         # shared engines must not interleave with another trial's
         self._lock = threading.RLock()
@@ -136,6 +203,9 @@ class GPSampler(_OptunaGPSampler):
             for engine in self._engines:
                 engine.close()
             self._engines = []
+            if self._ehvi_engine is not None:
+                self._ehvi_engine.close()
+                self._ehvi_engine = None
 
     def __del__(self) -> None:  # pragma: no cover
         try:
@@ -153,6 +223,15 @@ class GPSampler(_OptunaGPSampler):
         params = _fit(engine, X.shape[1], self._log_prior, self._minimum_noise,
                       None if cache is None else cache._params, self._deterministic)
         return _DeviceGP(engine, X, y, is_categorical, params)
+
+    def _device_ehvi(self, host: acqf_module.LogEHVI) -> acqf_module.BaseAcquisitionFunc:
+        """``host`` with its log-EHVI on the device, or ``host`` itself beyond the device's 24 objectives or when the
+        engine class answers only the GP calls (``_answers_ehvi``)."""
+        if host._fixed_samples.shape[-1] > _EHVI_MAX_OBJECTIVES or not _answers_ehvi(_engine_cls):
+            return host
+        if self._ehvi_engine is None:
+            self._ehvi_engine = _engine_cls(self._device)
+        return _DeviceLogEHVI(host, self._ehvi_engine)
 
     def _get_constraints_acqf_args(self, constraint_vals: np.ndarray,
                                    internal_search_space: gp_search_space.SearchSpace,
@@ -218,13 +297,13 @@ class GPSampler(_OptunaGPSampler):
                 )
                 best_params = normalized_params[np.argmax(standardized_score_vals), np.newaxis]
             else:
-                acqf = acqf_module.LogEHVI(
+                acqf = self._device_ehvi(acqf_module.LogEHVI(
                     gpr_list=gprs_list,
                     search_space=internal_search_space,
                     Y_train=torch.from_numpy(standardized_score_vals),
                     n_qmc_samples=128,
                     qmc_seed=self._rng.rng.randint(1 << 30),
-                )
+                ))
                 best_params = self._get_best_params_for_multi_objective(normalized_params, standardized_score_vals)
         else:
             constraint_vals, is_feasible = _get_constraint_vals_and_feasibility(study, completed_trials)
@@ -256,6 +335,8 @@ class GPSampler(_OptunaGPSampler):
                     constraints_gpr_list=constr_gpr_list,
                     constraints_threshold_list=constr_threshold_list,
                 )
+                if acqf._acqf is not None:   # None when no trial is feasible: the LogPI terms alone
+                    acqf._acqf = self._device_ehvi(acqf._acqf)
                 best_params = (
                     self._get_best_params_for_multi_objective(
                         normalized_params[is_feasible], standardized_score_vals[is_feasible]
