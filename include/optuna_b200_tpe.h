@@ -42,7 +42,8 @@ extern "C" {
 /* 11: + tpe_gp_loss_fixed_noise, tpe_gp_posterior_moments */
 /* 12: + tpe_gp_condition, tpe_gp_query */
 /* 13: + tpe_ehvi_set, tpe_ehvi */
-#define TPE_ABI_VERSION 13
+/* 14: + tpe_box_decomposition, tpe_get_box_decomposition */
+#define TPE_ABI_VERSION 14
 
 enum {
   TPE_OK = 0,
@@ -351,6 +352,19 @@ int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double
 int tpe_ehvi_set(tpe_ctx* ctx, const double* lower, const double* intervals, int64_t B, const double* samples,
                  int32_t S, int32_t M);
 int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, double* value, double* dmean, double* dsd);
+/* Non-dominated box decomposition of LogEHVI (get_non_dominated_box_bounds, optuna/_hypervolume/box_decomposition.py:
+ * 138-157, as optuna/_gp/acqf.py:255-263 calls it).  Kept apart from every other state of the context.
+ * tpe_box_decomposition decomposes the space that the rows of loss_vals [n, M] (minimised) do not dominate, below
+ * ref_point [M], into *n_boxes boxes and keeps them: the reference's arrays bit for bit, in its row order.  The one
+ * freedom is numpy's: of rows that np.unique merges because they differ only in the sign of a zero, which one it keeps.
+ * 2 <= M <= 24, n >= 1, loss values finite, no NaN in ref_point; TPE_E_INVALID naming the violated condition, or the
+ * bytes needed when the device lacks the memory of the bounds' pool.  *n_boxes = 0 is a valid result.
+ * tpe_get_box_decomposition copies out the last decomposition: lower, upper [n_boxes, M] (each may be NULL) and, if
+ * stats is non-NULL, stats[6] = the front's size, the first pass's bounds made and kept, the second pass's front,
+ * bounds made and kept.  TPE_E_STATE before a successful tpe_box_decomposition. */
+int tpe_box_decomposition(tpe_ctx* ctx, const double* loss_vals, int64_t n, int32_t M, const double* ref_point,
+                          int64_t* n_boxes);
+int tpe_get_box_decomposition(tpe_ctx* ctx, double* lower, double* upper, int64_t* stats);
 /* Candidates / log-densities of the last tpe_sample_and_select (all asks).
  * samples [n_asks * C, n_cols]; logl, logg [n_asks * C].  Any pointer may be NULL. */
 int tpe_get_candidates(tpe_ctx* ctx, double* samples, double* logl, double* logg);

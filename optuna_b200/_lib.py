@@ -83,6 +83,8 @@ SYMBOLS = {
     "tpe_gp_query": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P, _P]),
     "tpe_ehvi_set": (C.c_int, [_P, _P, _P, C.c_int64, _P, C.c_int32, C.c_int32]),
     "tpe_ehvi": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, _P]),
+    "tpe_box_decomposition": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.POINTER(C.c_int64)]),
+    "tpe_get_box_decomposition": (C.c_int, [_P, _P, _P, _P]),
     "tpe_get_candidates": (C.c_int, [_P, _P, _P, _P]),
     "tpe_logpdf": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P]),
     "tpe_last_timing": (C.c_int, [_P, _P, _P]),
@@ -93,7 +95,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 13  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 14  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

@@ -24,6 +24,7 @@
 #include "tpe_fanova.cuh"
 #include "tpe_gp.cuh"
 #include "tpe_ehvi.cuh"
+#include "tpe_boxdec.cuh"
 #include "tpe_uni.cuh"
 #include "tpe_mixed.cuh"
 #include "tpe_tcscreen.cuh"
@@ -146,6 +147,23 @@ struct EhviState {
   void release() {
     for (DevBuf* b : {&lbI, &Z, &mean, &sd, &part, &value, &dmean, &dsd}) b->release();
     *this = EhviState();
+  }
+};
+
+// non-dominated box decomposition (tpe_box_decomposition, tpe_boxdec.cuh): the pool of k_bd_pass (cap bounds, kept
+// across calls), the sorting and selection scratch, and the result of the last call on the host
+struct BoxDecState {
+  int64_t cap = 0;
+  DevBuf ub, dp, live, act, dlist, dmask, doff, stat;
+  DevBuf rows, ref, sorted, front, key, idx, work, keep, sel, cnt, lo, hi;
+  std::vector<double> lower, upper;
+  int64_t stats[6] = {0, 0, 0, 0, 0, 0};
+  bool ready = false;
+  void release() {
+    for (DevBuf* b : {&ub, &dp, &live, &act, &dlist, &dmask, &doff, &stat, &rows, &ref, &sorted, &front, &key, &idx,
+                      &work, &keep, &sel, &cnt, &lo, &hi})
+      b->release();
+    *this = BoxDecState();
   }
 };
 
@@ -284,6 +302,7 @@ struct tpe_ctx {
   int64_t uni_ord_K = -1;
   GpState gp;
   EhviState ehvi;
+  BoxDecState boxdec;
 };
 
 namespace {
@@ -1883,22 +1902,20 @@ struct PfScratch {
   }
 };
 
-int pareto_front_run(tpe_ctx* ctx, const double* values, int n, int M, uint8_t* on_front) {
+// Pareto-front flags of the device rows d_v [n, M] into b.flags (n >= 1); b's other buffers are sized here
+int pareto_front_device(tpe_ctx* ctx, PfScratch& b, const double* d_v, int n, int M) {
   cudaStream_t st = ctx->stream;
-  PfScratch b;
   const size_t vb = (size_t)n * M * 8;
-  for (DevBuf* x : {&b.v, &b.s, &b.fv}) CU(x->ensure(vb));
+  for (DevBuf* x : {&b.s, &b.fv}) CU(x->ensure(vb));
   CU(b.s0.ensure((size_t)n * 8));
   CU(b.key.ensure((size_t)n * 16));
   CU(b.idx.ensure((size_t)n * 12));
   CU(b.work.ensure(sizeof(SortWork)));
   for (DevBuf* x : {&b.dom, &b.flags}) CU(x->ensure((size_t)n));
   CU(b.nf.ensure(4));
-  CU(cudaMemcpyAsync(b.v.p, values, vb, cudaMemcpyHostToDevice, st));
   for (DevBuf* x : {&b.dom, &b.flags}) CU(cudaMemsetAsync(x->p, 0, (size_t)n, st));
   CU(cudaMemsetAsync(b.nf.p, 0, 4, st));
   // 1. stable order by coordinate 0
-  const double* d_v = b.v.as<double>();
   int32_t pc = M;
   int j_col = 0, n_i = n;
   uint64_t* ka = b.key.as<uint64_t>();
@@ -1938,8 +1955,198 @@ int pareto_front_run(tpe_ctx* ctx, const double* values, int n, int M, uint8_t* 
                                     b.nf.as<int>(), b.flags.as<uint8_t>());
     CU(cudaGetLastError());
   }
+  return TPE_OK;
+}
+
+int pareto_front_run(tpe_ctx* ctx, const double* values, int n, int M, uint8_t* on_front) {
+  cudaStream_t st = ctx->stream;
+  PfScratch b;
+  const size_t vb = (size_t)n * M * 8;
+  CU(b.v.ensure(vb));
+  CU(cudaMemcpyAsync(b.v.p, values, vb, cudaMemcpyHostToDevice, st));
+  const int rc = pareto_front_device(ctx, b, b.v.as<double>(), n, M);
+  if (rc != TPE_OK) return rc;
   CU(cudaMemcpyAsync(on_front, b.flags.p, (size_t)n, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
+// ---- non-dominated box decomposition (tpe_boxdec.cuh) -------------------------------------------
+// bytes of the pool per bound: upper bound, defining points, live flag, and the active list (two), dominated list,
+// masks and offsets of k_bd_pass
+static size_t bd_bytes_per_bound(int M) { return (size_t)8 * M * (M + 1) + 1 + 5 * 4; }
+
+static int bd_oom(tpe_ctx* ctx, int64_t bounds, int M) {
+  cudaGetLastError();   // an allocation failure is not sticky; clear it
+  size_t free_b = 0, total_b = 0;
+  cudaMemGetInfo(&free_b, &total_b);
+  return fail(ctx, TPE_E_INVALID, "box decomposition: a pool of %lld bounds in %d objectives needs %zu bytes of device "
+              "memory (%zu free)", (long long)bounds, M, (size_t)bounds * bd_bytes_per_bound(M), free_b);
+}
+
+#define BD_ALLOC(buf, bytes, bounds)                                          \
+  do {                                                                        \
+    cudaError_t e_ = (buf).ensure(bytes);                                     \
+    if (e_ == cudaErrorMemoryAllocation) return bd_oom(ctx, (bounds), M);     \
+    CU(e_);                                                                   \
+  } while (0)
+
+// *count = number of keep[0, n) set, sel[0, *count) their positions (k_bd_select); synchronises
+static int bd_select(tpe_ctx* ctx, const uint8_t* keep, int n, int32_t* sel, int* count) {
+  BoxDecState& d = ctx->boxdec;
+  cudaStream_t st = ctx->stream;
+  boxdec::k_bd_select<<<1, boxdec::THREADS, 0, st>>>(keep, n, sel, d.cnt.as<int>());
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(count, d.cnt.p, 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
+// d.front [*nf, M] = the Pareto front of the rows d_rows [n, M] in np.unique(axis=0) order (box_decomposition.py:
+// 143-146 and 120-129): a lexicographic order by M stable radix passes, last column first; the rows that differ from
+// their predecessor; the Pareto filter of tpe_pareto.cuh over those.  Uses d.sorted, d.key, d.idx, d.work, d.keep,
+// d.sel.
+static int bd_sorted_front(tpe_ctx* ctx, const double* d_rows, int n, int M, int* nf) {
+  BoxDecState& d = ctx->boxdec;
+  cudaStream_t st = ctx->stream;
+  BD_ALLOC(d.key, (size_t)n * 16, n);
+  BD_ALLOC(d.idx, (size_t)n * 20, n);
+  BD_ALLOC(d.work, sizeof(SortWork), n);
+  BD_ALLOC(d.keep, (size_t)n, n);
+  BD_ALLOC(d.sel, (size_t)n * 4, n);
+  BD_ALLOC(d.sorted, (size_t)n * M * 8, n);
+  uint64_t* ka = d.key.as<uint64_t>();
+  uint64_t* kb = ka + n;
+  int32_t* ia = d.idx.as<int32_t>();
+  int32_t* ib = ia + n;
+  int32_t* ord[2] = {ib + n, ib + 2 * n};
+  SortWork* wk = d.work.as<SortWork>();
+  int G = std::max(1, std::min(std::min(ctx->sm_count, 160), (n + 1023) / 1024));
+  if (ctx->sort_cta_cap > 0) G = std::min(G, ctx->sort_cta_cap);
+  int32_t pc = M, n_i = n;
+  const int32_t* perm = nullptr;
+  int32_t* out = nullptr;
+  for (int j = M - 1; j >= 0; --j) {
+    out = ord[j & 1];
+    int j_col = j;
+    void* args[] = {&d_rows, &pc, &j_col, &n_i, &ka, &kb, &ia, &ib, &wk, &out, &perm};
+    CU(cudaLaunchCooperativeKernel((const void*)k_radix_sort_coop_perm, dim3(G), dim3(512), args, 0, st));
+    perm = out;
+  }
+  const int32_t* order = out;
+  boxdec::k_bd_unique<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(d_rows, order, n, M, d.keep.as<uint8_t>());
+  CU(cudaGetLastError());
+  int nu = 0;
+  int rc = bd_select(ctx, d.keep.as<uint8_t>(), n, d.sel.as<int32_t>(), &nu);
+  if (rc != TPE_OK) return rc;
+  const int64_t nm = (int64_t)nu * M;
+  boxdec::k_bd_gather<<<(unsigned)((nm + 255) / 256), 256, 0, st>>>(d_rows, order, d.sel.as<int32_t>(), nu, M, false,
+                                                                    d.sorted.as<double>());
+  CU(cudaGetLastError());
+  PfScratch pf;
+  rc = pareto_front_device(ctx, pf, d.sorted.as<double>(), nu, M);
+  if (rc != TPE_OK) return rc;
+  rc = bd_select(ctx, pf.flags.as<uint8_t>(), nu, d.sel.as<int32_t>(), nf);
+  if (rc != TPE_OK) return rc;
+  BD_ALLOC(d.front, (size_t)*nf * M * 8, n);
+  const int64_t fm = (int64_t)*nf * M;
+  boxdec::k_bd_gather<<<(unsigned)((fm + 255) / 256), 256, 0, st>>>(d.sorted.as<double>(), nullptr, d.sel.as<int32_t>(),
+                                                                    *nf, M, false, d.front.as<double>());
+  CU(cudaGetLastError());
+  return TPE_OK;
+}
+
+// one _get_upper_bound_set pass over d.front [nf, M] from d.ref: the pool's first *pool bounds, *live_n of them live
+// and listed in d.sel.  A pass that overflows the pool is run again on a pool four times larger.
+static int bd_pass(tpe_ctx* ctx, int nf, int M, int* pool, int* live_n) {
+  BoxDecState& d = ctx->boxdec;
+  cudaStream_t st = ctx->stream;
+  if (d.cap == 0) d.cap = 4096;
+  for (;;) {
+    const int64_t cap = d.cap;
+    BD_ALLOC(d.ub, (size_t)cap * M * 8, cap);
+    BD_ALLOC(d.dp, (size_t)cap * M * M * 8, cap);
+    BD_ALLOC(d.live, (size_t)cap, cap);
+    BD_ALLOC(d.act, (size_t)cap * 8, cap);
+    BD_ALLOC(d.dlist, (size_t)cap * 4, cap);
+    BD_ALLOC(d.dmask, (size_t)cap * 4, cap);
+    BD_ALLOC(d.doff, (size_t)cap * 4, cap);
+    BD_ALLOC(d.sel, (size_t)cap * 4, cap);
+    BD_ALLOC(d.keep, (size_t)cap, cap);
+    int32_t* act = d.act.as<int32_t>();
+    boxdec::k_bd_pass<<<1, boxdec::THREADS, 0, st>>>(d.front.as<double>(), nf, M, d.ref.as<double>(), d.ub.as<double>(),
+                                                     d.dp.as<double>(), d.live.as<uint8_t>(), act, act + cap,
+                                                     d.dlist.as<int32_t>(), d.dmask.as<uint32_t>(),
+                                                     d.doff.as<int32_t>(), (int)cap, d.stat.as<int>());
+    CU(cudaGetLastError());
+    int stat[2];
+    CU(cudaMemcpyAsync(stat, d.stat.p, 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+    if (stat[1] == 0) {
+      *pool = stat[0];
+      return bd_select(ctx, d.live.as<uint8_t>(), stat[0], d.sel.as<int32_t>(), live_n);
+    }
+    if (cap >= INT32_MAX / 4) return bd_oom(ctx, cap * 4, M);
+    d.cap = cap * 4;
+  }
+}
+
+// get_non_dominated_box_bounds (box_decomposition.py:138-157) of d.rows [n, M] against ref [M]: d.lower, d.upper
+static int bd_run(tpe_ctx* ctx, int n, int M, const double* ref) {
+  BoxDecState& d = ctx->boxdec;
+  cudaStream_t st = ctx->stream;
+  CU(d.ref.ensure((size_t)M * 8));
+  CU(d.cnt.ensure(4));
+  CU(d.stat.ensure(8));
+  // 1. the front of the unique-lexsorted rows; 2. pass 1
+  int nf1 = 0, pool1 = 0, live1 = 0;
+  int rc = bd_sorted_front(ctx, d.rows.as<double>(), n, M, &nf1);
+  if (rc != TPE_OK) return rc;
+  CU(cudaMemcpyAsync(d.ref.p, ref, (size_t)M * 8, cudaMemcpyHostToDevice, st));
+  rc = bd_pass(ctx, nf1, M, &pool1, &live1);
+  if (rc != TPE_OK) return rc;
+  // 3. the negated upper bounds, their unique-lexsorted front; 4. pass 2 from +inf
+  BD_ALLOC(d.rows, (size_t)live1 * M * 8, live1);
+  const int64_t lm = (int64_t)live1 * M;
+  boxdec::k_bd_gather<<<(unsigned)((lm + 255) / 256), 256, 0, st>>>(d.ub.as<double>(), nullptr, d.sel.as<int32_t>(),
+                                                                    live1, M, true, d.rows.as<double>());
+  CU(cudaGetLastError());
+  int nf2 = 0, pool2 = 0, live2 = 0;
+  rc = bd_sorted_front(ctx, d.rows.as<double>(), live1, M, &nf2);
+  if (rc != TPE_OK) return rc;
+  const std::vector<double> inf((size_t)M, INFINITY);
+  CU(cudaMemcpyAsync(d.ref.p, inf.data(), (size_t)M * 8, cudaMemcpyHostToDevice, st));
+  rc = bd_pass(ctx, nf2, M, &pool2, &live2);
+  if (rc != TPE_OK) return rc;
+  // 5. the boxes of the final bounds, the empty ones dropped
+  // (lo and hi hold the boxes of every final bound, then the kept ones behind them)
+  BD_ALLOC(d.lo, (size_t)live2 * M * 16, live2);
+  BD_ALLOC(d.hi, (size_t)live2 * M * 16, live2);
+  double* lo = d.lo.as<double>();
+  double* hi = d.hi.as<double>();
+  boxdec::k_bd_boxes<<<(unsigned)((live2 + 255) / 256), 256, 0, st>>>(d.ub.as<double>(), d.dp.as<double>(),
+                                                                      d.sel.as<int32_t>(), live2, M, lo, hi,
+                                                                      d.keep.as<uint8_t>());
+  CU(cudaGetLastError());
+  int B = 0;
+  rc = bd_select(ctx, d.keep.as<uint8_t>(), live2, d.sel.as<int32_t>(), &B);
+  if (rc != TPE_OK) return rc;
+  d.lower.assign((size_t)B * M, 0.0);
+  d.upper.assign((size_t)B * M, 0.0);
+  if (B > 0) {
+    const int64_t bm = (int64_t)B * M;
+    const unsigned g = (unsigned)((bm + 255) / 256);
+    double* lo_kept = lo + (size_t)live2 * M;
+    double* hi_kept = hi + (size_t)live2 * M;
+    boxdec::k_bd_gather<<<g, 256, 0, st>>>(lo, nullptr, d.sel.as<int32_t>(), B, M, false, lo_kept);
+    boxdec::k_bd_gather<<<g, 256, 0, st>>>(hi, nullptr, d.sel.as<int32_t>(), B, M, false, hi_kept);
+    CU(cudaGetLastError());
+    CU(cudaMemcpyAsync(d.lower.data(), lo_kept, (size_t)bm * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaMemcpyAsync(d.upper.data(), hi_kept, (size_t)bm * 8, cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));
+  }
+  const int64_t stats[6] = {nf1, pool1 - 1, live1, nf2, pool2 - 1, live2};
+  std::copy(stats, stats + 6, d.stats);
   return TPE_OK;
 }
 
@@ -2244,6 +2451,7 @@ void tpe_ctx_destroy(tpe_ctx* ctx) {
   ctx->est[1].release();
   ctx->gp.release();
   ctx->ehvi.release();
+  ctx->boxdec.release();
   if (ctx->res_host) cudaFreeHost(ctx->res_host);
   if (ctx->mt_host) cudaFreeHost(ctx->mt_host);
   if (ctx->up_host) cudaFreeHost(ctx->up_host);
@@ -4020,6 +4228,45 @@ int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, doub
     CU(cudaMemcpyAsync(dsd, e.dsd.p, (size_t)Q * M * 8, cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
+// replaces get_non_dominated_box_bounds (optuna/_hypervolume/box_decomposition.py:138-157), as LogEHVI.__init__ calls
+// it (optuna/_gp/acqf.py:255-263)
+int tpe_box_decomposition(tpe_ctx* ctx, const double* loss_vals, int64_t n, int32_t M, const double* ref_point,
+                          int64_t* n_boxes) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  BoxDecState& d = ctx->boxdec;
+  d.ready = false;
+  if (M < 2 || M > boxdec::MAX_M)
+    return fail(ctx, TPE_E_INVALID, "box decomposition needs 2 <= M <= %d objectives, got %d", boxdec::MAX_M, M);
+  if (n < 1 || n >= (1ll << 31) - 4096)
+    return fail(ctx, TPE_E_INVALID, "box decomposition needs 1 <= n < 2^31 - 4096 rows, got %lld", (long long)n);
+  if (!loss_vals || !ref_point || !n_boxes) return fail(ctx, TPE_E_INVALID, "bad box decomposition arguments");
+  for (int64_t q = 0; q < n * M; ++q)
+    if (!std::isfinite(loss_vals[q]))
+      return fail(ctx, TPE_E_INVALID, "box decomposition: loss values must be finite (row %lld)", (long long)(q / M));
+  for (int j = 0; j < M; ++j)
+    if (std::isnan(ref_point[j])) return fail(ctx, TPE_E_INVALID, "box decomposition: the reference point holds a NaN");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  BD_ALLOC(d.rows, (size_t)n * M * 8, n);
+  CU(cudaMemcpyAsync(d.rows.p, loss_vals, (size_t)n * M * 8, cudaMemcpyHostToDevice, ctx->stream));
+  const int rc = bd_run(ctx, (int)n, M, ref_point);
+  if (rc != TPE_OK) return rc;
+  *n_boxes = (int64_t)(d.lower.size() / M);
+  d.ready = true;
+  return TPE_OK;
+}
+
+int tpe_get_box_decomposition(tpe_ctx* ctx, double* lower, double* upper, int64_t* stats) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  const BoxDecState& d = ctx->boxdec;
+  if (!d.ready) return fail(ctx, TPE_E_STATE, "no box decomposition (tpe_box_decomposition)");
+  if (lower) std::copy(d.lower.begin(), d.lower.end(), lower);
+  if (upper) std::copy(d.upper.begin(), d.upper.end(), upper);
+  if (stats) std::copy(d.stats, d.stats + 6, stats);
   return TPE_OK;
 }
 

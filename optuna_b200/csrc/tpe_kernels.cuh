@@ -344,7 +344,8 @@ struct SortWork {
 };
 __device__ __forceinline__ void d_radix_sort_coop(const double* __restrict__ mu, int32_t pc, int j_col, int n, uint64_t* __restrict__ key_a,
                   uint64_t* __restrict__ key_b, int32_t* __restrict__ idx_a, int32_t* __restrict__ idx_b,
-                  SortWork* __restrict__ wk, int32_t* __restrict__ order, const int* __restrict__ run_flag) {
+                  SortWork* __restrict__ wk, int32_t* __restrict__ order, const int* __restrict__ run_flag,
+                  const int32_t* __restrict__ perm = nullptr) {
   // run_flag != nullptr: the order may already have been brought up to date incrementally (k_order_update);
   // every CTA reads the same word before the first grid.sync
   if (run_flag != nullptr && *run_flag < 2) return;
@@ -356,9 +357,12 @@ __device__ __forceinline__ void d_radix_sort_coop(const double* __restrict__ mu,
   const int G = gridDim.x, b = blockIdx.x;
   const int chunk = (n + G - 1) / G;
   const int lo = min(n, b * chunk), hi = min(n, lo + chunk);
+  // perm != nullptr: sort the rows perm[0, n) (stable in that order), so that sorts by successive columns chain into
+  // a lexicographic order
   for (int i = lo + tid; i < hi; i += blockDim.x) {
-    key_a[i] = order_bits(mu[(int64_t)i * pc + j_col]);
-    idx_a[i] = i;
+    const int32_t r = perm != nullptr ? perm[i] : i;
+    key_a[i] = order_bits(mu[(int64_t)r * pc + j_col]);
+    idx_a[i] = r;
   }
   uint64_t* kin = key_a;
   uint64_t* kout = key_b;
@@ -432,6 +436,10 @@ __global__ void __launch_bounds__(512, 1)
 k_radix_sort_coop(const double* __restrict__ mu, int32_t pc, int j_col, int n, uint64_t* __restrict__ key_a,
                   uint64_t* __restrict__ key_b, int32_t* __restrict__ idx_a, int32_t* __restrict__ idx_b,
                   SortWork* __restrict__ wk, int32_t* __restrict__ order, const int* __restrict__ run_flag) { d_radix_sort_coop(mu, pc, j_col, n, key_a, key_b, idx_a, idx_b, wk, order, run_flag); }
+__global__ void __launch_bounds__(512, 1)
+k_radix_sort_coop_perm(const double* __restrict__ mu, int32_t pc, int j_col, int n, uint64_t* __restrict__ key_a,
+                       uint64_t* __restrict__ key_b, int32_t* __restrict__ idx_a, int32_t* __restrict__ idx_b,
+                       SortWork* __restrict__ wk, int32_t* __restrict__ order, const int32_t* __restrict__ perm) { d_radix_sort_coop(mu, pc, j_col, n, key_a, key_b, idx_a, idx_b, wk, order, nullptr, perm); }
 
 // Incremental maintenance of a column's sorted order between two suggestions (univariate TPE): the above set of the
 // next trial is almost always the previous one plus the trial that has just finished.

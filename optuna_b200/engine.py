@@ -531,6 +531,26 @@ class TPEEngine:
         self._check(self._lib.tpe_ehvi(self._h, _ptr(m), _ptr(s), m.shape[0], _ptr(value), _ptr(dmean), _ptr(dsd)))
         return (value, dmean, dsd) if grad else value
 
+    def box_decomposition(self, loss_vals, ref_point) -> tuple[np.ndarray, np.ndarray]:
+        """``get_non_dominated_box_bounds(loss_vals, ref_point)`` (optuna/_hypervolume/box_decomposition.py:138-157)
+        without its warning: ``(lower, upper)`` [B, M], the reference's bits in its row order (tpe_box_decomposition).
+        ``loss_vals`` [n, M] finite, minimised; ``ref_point`` [M] without NaN; 2 <= M <= 24.  B may be 0.  The counts
+        of the last call (front size, bounds made and kept by each pass) are in ``last_box_stats``.  Leaves every
+        other state of this engine unchanged."""
+        v, r = _f64(loss_vals), _f64(ref_point).reshape(-1)
+        if v.ndim != 2 or v.shape[1] != r.size:
+            raise ValueError(f"loss_vals must be [n, {r.size}] for a reference point of {r.size} objectives, got shape "
+                             f"{v.shape}")
+        n_boxes = C.c_int64()
+        self._check(self._lib.tpe_box_decomposition(self._h, _ptr(v), v.shape[0], v.shape[1], _ptr(r),
+                                                    C.byref(n_boxes)))
+        lower = np.empty((n_boxes.value, r.size))
+        upper = np.empty((n_boxes.value, r.size))
+        stats = np.empty(6, dtype=np.int64)
+        self._check(self._lib.tpe_get_box_decomposition(self._h, _ptr(lower), _ptr(upper), _ptr(stats)))
+        self.last_box_stats = dict(zip(("front", "born1", "bounds1", "front2", "born2", "bounds2"), stats.tolist()))
+        return lower, upper
+
     # -- inspection --------------------------------------------------------------------------------
     def get_split(self) -> tuple[np.ndarray, np.ndarray]:
         below = np.empty(self._info[1], dtype=np.int64)

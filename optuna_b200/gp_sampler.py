@@ -15,25 +15,34 @@ posterior's gradient in x against that factor (``TPEEngine.gp_condition`` / ``gp
 
 With two or more objectives the log-EHVI of ``LogEHVI`` (acqf.py:45-62, 245-300), and of ``ConstrainedLogEHVI``'s
 objective part, also runs on the device (``TPEEngine.ehvi_set`` / ``ehvi``): optuna builds a (points, 128 samples,
-boxes, objectives) fp64 tensor per evaluation, which at four objectives and a thousand trials is tens of GB.  optuna
-still computes the box decomposition, the QMC samples and the constraints' ``LogPI`` terms on the host; the other
-acquisition functions run unchanged over the device GPs.  Beyond 24 objectives optuna's host ``LogEHVI`` is kept.
+boxes, objectives) fp64 tensor per evaluation, which at four objectives and a thousand trials is tens of GB.  So does
+the non-dominated box decomposition ``LogEHVI.__init__`` computes once per ask (``TPEEngine.box_decomposition``):
+optuna's (optuna/_hypervolume/box_decomposition.py) costs seconds to minutes from five objectives on.  The device
+returns the reference's boxes bit for bit and in its order, so the acquisition is the one optuna builds.  optuna still
+computes the Pareto filter and reference point before the decomposition, the QMC samples and the constraints' ``LogPI``
+terms on the host; the other acquisition functions run unchanged over the device GPs.  Beyond 24 objectives optuna's
+host ``LogEHVI`` is kept.
 
-One difference: the device holds two n x n fp64 matrices per GP, and ``sample_relative`` raises ``ValueError``
-naming the need when the device lacks that memory.
+One difference: the device holds two n x n fp64 matrices per GP and a pool of the decomposition's bounds, and
+``sample_relative`` raises ``ValueError`` naming the need when the device lacks that memory.
 """
 from __future__ import annotations
 
+import os
+import sys
 import threading
+import warnings
 from typing import Any
 
 import numpy as np
 import torch
 from optuna._gp import acqf as acqf_module
 from optuna._gp import search_space as gp_search_space
+from optuna._warnings import _OPTUNA_MODULE_ROOT, optuna_warn
 from optuna.samplers import GPSampler as _OptunaGPSampler
 from optuna.samplers._gp.sampler import EPS, _get_constraint_vals_and_feasibility, _standardize_values
 from optuna.study import StudyDirection
+from optuna.study._multi_objective import _is_pareto_front
 
 from .engine import GPCholeskyError, TPEEngine
 from .terminator import _fit
@@ -50,6 +59,27 @@ def _answers_ehvi(engine_cls) -> bool:
     kernel is an error.  A substitute engine that restates only the GP calls (a host implementation of them) leaves the
     acquisition to optuna's host ``LogEHVI``, as before the device log-EHVI existed."""
     return callable(getattr(engine_cls, "ehvi_set", None)) and callable(getattr(engine_cls, "ehvi", None))
+
+
+def _answers_box_decomposition(engine_cls) -> bool:
+    """Whether ``engine_cls`` answers the box decomposition (``box_decomposition``).  ``TPEEngine`` always does; a
+    substitute engine without it leaves the decomposition to optuna's host ``LogEHVI``."""
+    return callable(getattr(engine_cls, "box_decomposition", None))
+
+
+_PACKAGE_ROOT = os.path.dirname(os.path.abspath(__file__)) + os.sep
+_BOX_DECOMPOSITION_WARNING = ("Box decomposition (typically used by `GPSampler`) might be significantly slow for "
+                              "n_objectives > 4. Please consider using another sampler instead.")
+
+
+def _warn_box_decomposition() -> None:
+    """The warning optuna's ``get_non_dominated_box_bounds`` emits for more than four objectives
+    (box_decomposition.py:151-155), attributed as ``optuna_warn`` attributes it: to the first frame outside optuna and
+    outside this package, so that warning filters match it as they match the reference's."""
+    if sys.version_info >= (3, 12):
+        warnings.warn(_BOX_DECOMPOSITION_WARNING, UserWarning, skip_file_prefixes=(_OPTUNA_MODULE_ROOT, _PACKAGE_ROOT))
+    else:  # pragma: no cover
+        optuna_warn(_BOX_DECOMPOSITION_WARNING)
 
 
 def _condition(engine, params: np.ndarray) -> None:
@@ -167,12 +197,13 @@ class GPSampler(_OptunaGPSampler):
     since the trials share those engines.
 
     With 2 to 24 objectives the log-EHVI acquisition (with constraints, its hypervolume part) is also evaluated on
-    the device, by one more engine kept across trials; optuna's other acquisition functions run unchanged over the
+    the device, by one more engine kept across trials, which also computes the acquisition's non-dominated box
+    decomposition: the reference's boxes, bit for bit.  optuna's other acquisition functions run unchanged over the
     device GPs.
 
     The device holds two n x n fp64 matrices per GP, n being the number of complete trials (plus the running ones in a
-    single-objective study without constraints).  When it lacks that memory, ``sample_relative`` raises
-    ``ValueError`` naming the need; this is the one difference from the reference.
+    single-objective study without constraints), and the bounds of the box decomposition.  When it lacks that memory,
+    ``sample_relative`` raises ``ValueError`` naming the need; this is the one difference from the reference.
 
     Args:
         seed: Random seed.
@@ -232,6 +263,38 @@ class GPSampler(_OptunaGPSampler):
         if self._ehvi_engine is None:
             self._ehvi_engine = _engine_cls(self._device)
         return _DeviceLogEHVI(host, self._ehvi_engine)
+
+    def _log_ehvi(self, gpr_list: list[_DeviceGP], search_space: gp_search_space.SearchSpace, Y_train: np.ndarray,
+                  qmc_seed: int) -> acqf_module.BaseAcquisitionFunc:
+        """``LogEHVI(gpr_list, search_space, Y_train, 128, qmc_seed)`` through ``_device_ehvi``.  When the engine class
+        answers the box decomposition and the EHVI calls and there are at most 24 objectives, the ``LogEHVI`` is built
+        as acqf.py:255-280 builds it, with the decomposition on the device: the same Pareto filter and reference point
+        on the host, the device's boxes flipped back to maximisation, the same clamp, samples and length scales."""
+        M = Y_train.shape[-1]
+        if M > _EHVI_MAX_OBJECTIVES or not (_answers_ehvi(_engine_cls) and _answers_box_decomposition(_engine_cls)):
+            return self._device_ehvi(acqf_module.LogEHVI(gpr_list=gpr_list, search_space=search_space,
+                                                         Y_train=torch.from_numpy(Y_train), n_qmc_samples=128,
+                                                         qmc_seed=qmc_seed))
+        if self._ehvi_engine is None:
+            self._ehvi_engine = _engine_cls(self._device)
+        host = acqf_module.LogEHVI.__new__(acqf_module.LogEHVI)
+        host._stabilizing_noise = 1e-12
+        host._gpr_list = gpr_list
+        host._fixed_samples = acqf_module._sample_from_normal_sobol(dim=M, n_samples=128, seed=qmc_seed)
+        # acqf.py:257-263: Y is maximised, loss_vals minimised
+        loss_vals = -Y_train
+        pareto_sols = loss_vals[_is_pareto_front(loss_vals, assume_unique_lexsorted=False)]
+        ref_point = np.max(loss_vals, axis=0)
+        ref_point = np.nextafter(np.maximum(1.1 * ref_point, 0.9 * ref_point), np.inf)
+        if M > 4:
+            _warn_box_decomposition()
+        lbs, ubs = self._ehvi_engine.box_decomposition(pareto_sols, ref_point)
+        host._non_dominated_box_lower_bounds = torch.from_numpy(-ubs)
+        upper = torch.from_numpy(-lbs)
+        host._non_dominated_box_intervals = (upper - host._non_dominated_box_lower_bounds).clamp_min_(acqf_module._EPS)
+        acqf_module.BaseAcquisitionFunc.__init__(host, np.mean([gpr.length_scales for gpr in gpr_list], axis=0),
+                                                 search_space)
+        return self._device_ehvi(host)
 
     def _get_constraints_acqf_args(self, constraint_vals: np.ndarray,
                                    internal_search_space: gp_search_space.SearchSpace,
@@ -297,13 +360,8 @@ class GPSampler(_OptunaGPSampler):
                 )
                 best_params = normalized_params[np.argmax(standardized_score_vals), np.newaxis]
             else:
-                acqf = self._device_ehvi(acqf_module.LogEHVI(
-                    gpr_list=gprs_list,
-                    search_space=internal_search_space,
-                    Y_train=torch.from_numpy(standardized_score_vals),
-                    n_qmc_samples=128,
-                    qmc_seed=self._rng.rng.randint(1 << 30),
-                ))
+                acqf = self._log_ehvi(gprs_list, internal_search_space, standardized_score_vals,
+                                      self._rng.rng.randint(1 << 30))
                 best_params = self._get_best_params_for_multi_objective(normalized_params, standardized_score_vals)
         else:
             constraint_vals, is_feasible = _get_constraint_vals_and_feasibility(study, completed_trials)
@@ -324,19 +382,20 @@ class GPSampler(_OptunaGPSampler):
                 best_params = None if np.isneginf(best_feasible_y) else normalized_params[i_opt, np.newaxis]
             else:
                 is_all_infeasible = not any(is_feasible)
+                qmc_seed = self._rng.rng.randint(1 << 30)
+                # built without its LogEHVI, which _log_ehvi builds as ConstrainedLogEHVI would (acqf.py:318-322)
                 acqf = acqf_module.ConstrainedLogEHVI(
                     gpr_list=gprs_list,
                     search_space=internal_search_space,
-                    Y_feasible=(
-                        torch.from_numpy(standardized_score_vals[is_feasible]) if not is_all_infeasible else None
-                    ),
+                    Y_feasible=None,
                     n_qmc_samples=128,
-                    qmc_seed=self._rng.rng.randint(1 << 30),
+                    qmc_seed=qmc_seed,
                     constraints_gpr_list=constr_gpr_list,
                     constraints_threshold_list=constr_threshold_list,
                 )
-                if acqf._acqf is not None:   # None when no trial is feasible: the LogPI terms alone
-                    acqf._acqf = self._device_ehvi(acqf._acqf)
+                if not is_all_infeasible:   # else the LogPI terms alone
+                    acqf._acqf = self._log_ehvi(gprs_list, internal_search_space,
+                                                standardized_score_vals[is_feasible], qmc_seed)
                 best_params = (
                     self._get_best_params_for_multi_objective(
                         normalized_params[is_feasible], standardized_score_vals[is_feasible]
