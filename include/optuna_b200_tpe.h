@@ -43,7 +43,8 @@ extern "C" {
 /* 12: + tpe_gp_condition, tpe_gp_query */
 /* 13: + tpe_ehvi_set, tpe_ehvi */
 /* 14: + tpe_box_decomposition, tpe_get_box_decomposition */
-#define TPE_ABI_VERSION 14
+/* 15: + tpe_gp_batch_set, tpe_gp_batch_loss, tpe_gp_batch_bounds */
+#define TPE_ABI_VERSION 15
 
 enum {
   TPE_OK = 0,
@@ -336,6 +337,29 @@ int tpe_gp_posterior_moments(tpe_ctx* ctx, const double* params, const double* X
                              double* mean, double* var, double* cov);
 int tpe_gp_condition(tpe_ctx* ctx, const double* params);
 int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double* var, double* dmean, double* dvar);
+/* Many independent Gaussian processes at once, fp64: the per-prefix fits of plot_terminator_improvement
+ * (optuna/visualization/_terminator_improvement.py:83-132, one RegretBoundEvaluator.evaluate per trial).  Kept apart
+ * from the history, the suggestion state and the single-GP state.
+ * tpe_gp_batch_set sets n_gp GPs: GP i has the rows offsets[i] .. offsets[i + 1] - 1 of X [N, P] and y [N]
+ * (offsets [n_gp + 1], offsets[0] = 0, N = offsets[n_gp]), all share is_categorical [P].  n_gp >= 1, every
+ * n_i >= 1, P >= 1, X and y finite.  TPE_E_INVALID naming the bytes when the device lacks the memory for the data
+ * and one loss call over every GP.
+ * tpe_gp_batch_loss is tpe_gp_loss for k jobs: job b is GP gp_idx[b] at raw[b] [P + 2] (the raw parameters of
+ * tpe_gp_loss); loss[b] = -log p(y), grad[b] [P + 2].  status[b] = 0, or 1 when the kernel parameters are not finite
+ * or the covariance is not positive definite (tpe_gp_loss's TPE_E_NOTPD), with loss and grad NaN; the other jobs are
+ * unaffected.
+ * tpe_gp_batch_bounds: job b is GP gp_idx[b] at params[b] [P + 2] (inverse squared lengthscales, kernel scale,
+ * noise_var) with beta[b] >= 0 and the S sample rows samples[b] [S, P]; out[b] [3] = max over the GP's train rows of
+ * mean + sqrt(beta var), the same over the sample rows, and max over the train rows of mean - sqrt(beta var), var
+ * clamped at 0 and NaN propagating as np.max propagates it (RegretBoundEvaluator.evaluate, optuna/terminator/
+ * improvement/evaluator.py:50-84).  status as for the loss.
+ * Several jobs may name the same GP.  A job's outputs are the same bits whatever the other jobs of the call are. */
+int tpe_gp_batch_set(tpe_ctx* ctx, int32_t n_gp, const int64_t* offsets, int32_t P, const double* X, const double* y,
+                     const uint8_t* is_categorical);
+int tpe_gp_batch_loss(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* raw, double minimum_noise,
+                      double* loss, double* grad, int32_t* status);
+int tpe_gp_batch_bounds(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* params, const double* beta,
+                        int32_t S, const double* samples, double* out, int32_t* status);
 /* Log expected hypervolume improvement of GPSampler's multi-objective acquisition (LogEHVI, optuna/_gp/acqf.py:245-300,
  * with logehvi :45-62), fp64.  Kept apart from the history, the suggestion state and the GP state.
  * tpe_ehvi_set replaces the state LogEHVI.__init__ builds (acqf.py:245-280): lower [B, M] the lower bounds of the

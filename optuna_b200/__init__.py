@@ -8,7 +8,8 @@ from .engine import ParamSpec, TPEEngine  # noqa: F401
 
 __all__ = ["ParamSpec", "TPEEngine", "B200TPESampler", "hypervolume_history", "plot_hypervolume_history",
            "best_trials", "pareto_front_info", "plot_pareto_front", "FanovaImportanceEvaluator",
-           "RegretBoundEvaluator", "EMMREvaluator", "GPSampler"]
+           "RegretBoundEvaluator", "EMMREvaluator", "GPSampler", "terminator_improvement_history",
+           "plot_terminator_improvement"]
 
 
 def __getattr__(name):
@@ -22,9 +23,12 @@ def __getattr__(name):
     if name == "FanovaImportanceEvaluator":
         from .importance import FanovaImportanceEvaluator
         return FanovaImportanceEvaluator
-    if name in ("RegretBoundEvaluator", "EMMREvaluator"):
+    if name in ("RegretBoundEvaluator", "EMMREvaluator", "terminator_improvement_history"):
         from . import terminator
         return getattr(terminator, name)
+    if name == "plot_terminator_improvement":
+        from .analysis import plot_terminator_improvement
+        return plot_terminator_improvement
     if name == "GPSampler":
         from .gp_sampler import GPSampler
         return GPSampler

@@ -85,6 +85,9 @@ SYMBOLS = {
     "tpe_ehvi": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, _P]),
     "tpe_box_decomposition": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.POINTER(C.c_int64)]),
     "tpe_get_box_decomposition": (C.c_int, [_P, _P, _P, _P]),
+    "tpe_gp_batch_set": (C.c_int, [_P, C.c_int32, _P, C.c_int32, _P, _P, _P]),
+    "tpe_gp_batch_loss": (C.c_int, [_P, C.c_int64, _P, _P, C.c_double, _P, _P, _P]),
+    "tpe_gp_batch_bounds": (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, _P, _P, _P]),
     "tpe_get_candidates": (C.c_int, [_P, _P, _P, _P]),
     "tpe_logpdf": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P]),
     "tpe_last_timing": (C.c_int, [_P, _P, _P]),
@@ -95,7 +98,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 14  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 15  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

@@ -248,3 +248,19 @@ def plot_pareto_front(study, *, target_names: list[str] | None = None, include_d
     return _get_pareto_front_plot(pareto_front_info(
         study, target_names=target_names, include_dominated_trials=include_dominated_trials, axis_order=axis_order,
         constraints_func=constraints_func, targets=targets, device=device))
+
+
+def plot_terminator_improvement(study, plot_error: bool = False, improvement_evaluator=None, error_evaluator=None,
+                                min_n_trials: int = 20):
+    """Drop-in for ``optuna.visualization.plot_terminator_improvement``: the same ``plotly`` figure, with the
+    improvement of every trial prefix from ``optuna_b200.terminator_improvement_history`` (all prefixes' Gaussian
+    processes fitted together on the GPU for ``optuna_b200.RegretBoundEvaluator``, the default).  Needs plotly, as
+    optuna's does."""
+    from optuna.visualization._plotly_imports import _imports
+    from optuna.visualization._terminator_improvement import _get_improvement_plot
+
+    from .terminator import terminator_improvement_history
+
+    _imports.check()
+    info = terminator_improvement_history(study, improvement_evaluator, error_evaluator, get_error=plot_error)
+    return _get_improvement_plot(info, min_n_trials)

@@ -23,6 +23,7 @@
 #include "tpe_pareto.cuh"
 #include "tpe_fanova.cuh"
 #include "tpe_gp.cuh"
+#include "tpe_gpbatch.cuh"
 #include "tpe_ehvi.cuh"
 #include "tpe_boxdec.cuh"
 #include "tpe_uni.cuh"
@@ -134,6 +135,20 @@ struct GpState {
                     (void*)cat, (void*)fail})
       if (p) cudaFree(p);
     *this = GpState();
+  }
+};
+
+// Many Gaussian processes of one study at once (tpe_gp_batch_*, tpe_gpbatch.cuh): the packed data of
+// tpe_gp_batch_set, and the per-call buffers (jobs, per-job workspace, outputs) of the loss and bounds calls
+struct GpBatchState {
+  int32_t n_gp = 0, P = 0;
+  std::vector<int64_t> off;   // host copy of the row offsets [n_gp + 1]
+  DevBuf X, y, doff, cat, idx, prm, nexc, ws, wsoff, loss, grad, status, beta, Xs, out;
+  bool ready = false;
+  void release() {
+    for (DevBuf* b : {&X, &y, &doff, &cat, &idx, &prm, &nexc, &ws, &wsoff, &loss, &grad, &status, &beta, &Xs, &out})
+      b->release();
+    *this = GpBatchState();
   }
 };
 
@@ -301,6 +316,7 @@ struct tpe_ctx {
   int32_t uni_ord_col = -1;
   int64_t uni_ord_K = -1;
   GpState gp;
+  GpBatchState gpb;
   EhviState ehvi;
   BoxDecState boxdec;
 };
@@ -2450,6 +2466,7 @@ void tpe_ctx_destroy(tpe_ctx* ctx) {
   ctx->est[0].release();
   ctx->est[1].release();
   ctx->gp.release();
+  ctx->gpb.release();
   ctx->ehvi.release();
   ctx->boxdec.release();
   if (ctx->res_host) cudaFreeHost(ctx->res_host);
@@ -4125,6 +4142,203 @@ int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double
 }
 
 // ---- log-EHVI of GPSampler's multi-objective acquisition (tpe_ehvi.cuh) ----------------------------------------------
+// ---- Many Gaussian processes at once (tpe_gpbatch.cuh) -------------------------------------------------------------
+static size_t gpb_free_bytes(tpe_ctx* ctx) {
+  size_t free_b = 0, total_b = 0;
+  if (cudaMemGetInfo(&free_b, &total_b) != cudaSuccess) return 0;
+  return free_b;
+}
+
+// Per-job workspace offsets (doubles) of a call: k_gpb_loss needs gpb::ws_doubles(n), k_gpb_bounds also n x NQ
+// doubles of cross covariance.  Jobs get their own workspace even when they name the same GP.
+static int64_t gpb_ws_layout(const GpBatchState& s, const int32_t* gp_idx, int64_t k, bool bounds,
+                             std::vector<int64_t>& wsoff, size_t* smem) {
+  int64_t tot = 0;
+  *smem = 0;
+  wsoff.resize(k);
+  for (int64_t b = 0; b < k; ++b) {
+    const int64_t n = s.off[gp_idx[b] + 1] - s.off[gp_idx[b]];
+    wsoff[b] = tot;
+    tot += gpb::ws_doubles(n) + (bounds ? n * gpb::NQ : 0);
+    *smem = std::max(*smem, gpb::smem_bytes((int)n, s.P));
+  }
+  return tot;
+}
+
+static int gpb_check_jobs(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx) {
+  const GpBatchState& s = ctx->gpb;
+  if (!s.ready) return fail(ctx, TPE_E_STATE, "no batched GP data (tpe_gp_batch_set)");
+  if (k < 1 || !gp_idx) return fail(ctx, TPE_E_INVALID, "bad batched GP call (k %lld)", (long long)k);
+  for (int64_t b = 0; b < k; ++b)
+    if (gp_idx[b] < 0 || gp_idx[b] >= s.n_gp)
+      return fail(ctx, TPE_E_INVALID, "GP index %d out of range (%d GPs)", gp_idx[b], s.n_gp);
+  return TPE_OK;
+}
+
+static int gpb_oom(tpe_ctx* ctx, const char* what, size_t need, int64_t nmax) {
+  return fail(ctx, TPE_E_INVALID,
+              "%s needs %zu bytes (%.2f GB) of device memory (largest GP: n = %lld), device %d has %zu bytes free",
+              what, need, need / 1e9, (long long)nmax, ctx->device, gpb_free_bytes(ctx));
+}
+
+// Uploads the job list and sizes the per-job workspace and the launch's shared memory; the caller has checked the
+// jobs.  Fails naming the bytes when the workspace does not fit in free device memory.
+static int gpb_stage_jobs(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, bool bounds, size_t extra,
+                          size_t* smem) {
+  GpBatchState& s = ctx->gpb;
+  std::vector<int64_t> wsoff;
+  const int64_t wsd = gpb_ws_layout(s, gp_idx, k, bounds, wsoff, smem);
+  int64_t nmax = 0;
+  for (int64_t b = 0; b < k; ++b) nmax = std::max(nmax, s.off[gp_idx[b] + 1] - s.off[gp_idx[b]]);
+  const size_t need = (size_t)std::max<int64_t>(wsd, 1) * 8 + extra;
+  const size_t have = s.ws.cap;
+  if (need > have && need - have > gpb_free_bytes(ctx))
+    return gpb_oom(ctx, bounds ? "the batched GP bounds" : "the batched GP loss", need, nmax);
+  cudaStream_t st = ctx->stream;
+  CU(s.ws.ensure((size_t)std::max<int64_t>(wsd, 1) * 8));
+  CU(s.wsoff.ensure(k * 8));
+  CU(s.idx.ensure(k * 4));
+  CU(s.status.ensure(k * 4));
+  CU(cudaMemcpyAsync(s.wsoff.p, wsoff.data(), k * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.idx.p, gp_idx, k * 4, cudaMemcpyHostToDevice, st));
+  if (*smem > 48 * 1024) {
+    CU(cudaFuncSetAttribute(gpb::k_gpb_loss, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
+    CU(cudaFuncSetAttribute(gpb::k_gpb_bounds, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
+  }
+  return TPE_OK;
+}
+
+// n_gp Gaussian processes over the rows offsets[i] .. offsets[i + 1] - 1 of X [N, P] / y [N]
+int tpe_gp_batch_set(tpe_ctx* ctx, int32_t n_gp, const int64_t* offsets, int32_t P, const double* X, const double* y,
+                     const uint8_t* is_categorical) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  GpBatchState& s = ctx->gpb;
+  s.ready = false;
+  if (n_gp < 1) return fail(ctx, TPE_E_INVALID, "no GPs in the batch (n_gp %d)", n_gp);
+  if (P < 1) return fail(ctx, TPE_E_INVALID, "bad batched GP width (P %d)", P);
+  if (!offsets || !X || !y || !is_categorical) return fail(ctx, TPE_E_INVALID, "bad batched GP arguments");
+  if (offsets[0] != 0) return fail(ctx, TPE_E_INVALID, "batched GP offsets must start at 0");
+  int64_t nmax = 0, wsd = 0;
+  for (int32_t i = 0; i < n_gp; ++i) {
+    const int64_t n = offsets[i + 1] - offsets[i];
+    if (n < 1 || n > (int64_t)1 << 20)
+      return fail(ctx, TPE_E_INVALID, "GP %d of the batch has n = %lld rows (needs 1 .. 2^20)", i, (long long)n);
+    nmax = std::max(nmax, n);
+    wsd += gpb::ws_doubles(n);
+  }
+  const int64_t N = offsets[n_gp];
+  for (int64_t i = 0; i < N * P; ++i)
+    if (!std::isfinite(X[i])) return fail(ctx, TPE_E_INVALID, "batched GP inputs hold a non-finite value");
+  for (int64_t i = 0; i < N; ++i)
+    if (!std::isfinite(y[i])) return fail(ctx, TPE_E_INVALID, "batched GP targets hold a non-finite value");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  s.release();
+  // the data, and the workspace of one loss call over every GP (n x n fp64 per GP above the shared-memory size)
+  const size_t need = 8 * ((size_t)N * (P + 1) + (size_t)n_gp + 1 + (size_t)wsd) + P;
+  if (need > gpb_free_bytes(ctx)) return gpb_oom(ctx, "the batch of Gaussian processes", need, nmax);
+  cudaStream_t st = ctx->stream;
+  std::vector<uint8_t> cat(P);
+  for (int d = 0; d < P; ++d) cat[d] = is_categorical[d] ? 1 : 0;
+  s.n_gp = n_gp;
+  s.P = P;
+  s.off.assign(offsets, offsets + n_gp + 1);
+  CU(s.X.ensure((size_t)N * P * 8));
+  CU(s.y.ensure((size_t)N * 8));
+  CU(s.doff.ensure((size_t)(n_gp + 1) * 8));
+  CU(s.cat.ensure(P));
+  CU(cudaMemcpyAsync(s.X.p, X, (size_t)N * P * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.y.p, y, (size_t)N * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.doff.p, offsets, (size_t)(n_gp + 1) * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.cat.p, cat.data(), P, cudaMemcpyHostToDevice, st));
+  CU(cudaStreamSynchronize(st));
+  s.ready = true;
+  return TPE_OK;
+}
+
+// tpe_gp_loss for k jobs at once: job b is GP gp_idx[b] at raw[b] [P + 2]
+int tpe_gp_batch_loss(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* raw, double minimum_noise,
+                      double* loss, double* grad, int32_t* status) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  int rc = gpb_check_jobs(ctx, k, gp_idx);
+  if (rc != TPE_OK) return rc;
+  if (!raw || !loss || !grad || !status) return fail(ctx, TPE_E_INVALID, "bad batched GP loss arguments");
+  if (!std::isfinite(minimum_noise) || minimum_noise < 0.0) return fail(ctx, TPE_E_INVALID, "bad minimum noise");
+  GpBatchState& s = ctx->gpb;
+  const int P = s.P;
+  if (set_device(ctx)) return TPE_E_CUDA;
+  size_t smem = 0;
+  rc = gpb_stage_jobs(ctx, k, gp_idx, false, 0, &smem);
+  if (rc != TPE_OK) return rc;
+  // the kernel parameters as tpe_gp_loss forms them on the host; a non-finite one is reported by the kernel
+  std::vector<double> prm((size_t)k * (P + 2)), nexc(k);
+  for (int64_t b = 0; b < k; ++b) {
+    const double* r = raw + b * (P + 2);
+    double* p = prm.data() + b * (P + 2);
+    for (int d = 0; d <= P; ++d) p[d] = std::exp(r[d]);
+    nexc[b] = std::exp(r[P + 1]);
+    p[P + 1] = nexc[b] + minimum_noise;
+  }
+  cudaStream_t st = ctx->stream;
+  CU(s.prm.ensure(prm.size() * 8));
+  CU(s.nexc.ensure(k * 8));
+  CU(s.loss.ensure(k * 8));
+  CU(s.grad.ensure(prm.size() * 8));
+  CU(cudaMemcpyAsync(s.prm.p, prm.data(), prm.size() * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.nexc.p, nexc.data(), k * 8, cudaMemcpyHostToDevice, st));
+  gpb::k_gpb_loss<<<(unsigned)k, gpb::THREADS, smem, st>>>(
+      s.X.as<double>(), s.y.as<double>(), s.doff.as<int64_t>(), s.cat.as<uint8_t>(), P, s.idx.as<int32_t>(),
+      s.prm.as<double>(), s.nexc.as<double>(), s.ws.as<double>(), s.wsoff.as<int64_t>(), s.loss.as<double>(),
+      s.grad.as<double>(), s.status.as<int32_t>());
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(loss, s.loss.p, k * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(grad, s.grad.p, prm.size() * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(status, s.status.p, k * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
+// RegretBoundEvaluator's three maxima for k jobs: GP gp_idx[b] at params[b] [P + 2], beta[b], and its S sample rows
+// samples[b] [S, P]
+int tpe_gp_batch_bounds(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* params, const double* beta,
+                        int32_t S, const double* samples, double* out, int32_t* status) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  int rc = gpb_check_jobs(ctx, k, gp_idx);
+  if (rc != TPE_OK) return rc;
+  if (!params || !beta || !out || !status || S < 1 || !samples)
+    return fail(ctx, TPE_E_INVALID, "bad batched GP bounds arguments");
+  GpBatchState& s = ctx->gpb;
+  const int P = s.P;
+  for (int64_t b = 0; b < k; ++b)
+    if (!std::isfinite(beta[b]) || beta[b] < 0.0) return fail(ctx, TPE_E_INVALID, "bad beta");
+  const int64_t ns = k * (int64_t)S * P;
+  for (int64_t i = 0; i < ns; ++i)
+    if (!std::isfinite(samples[i])) return fail(ctx, TPE_E_INVALID, "sample points hold a non-finite value");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  size_t smem = 0;
+  rc = gpb_stage_jobs(ctx, k, gp_idx, true, (size_t)ns * 8, &smem);
+  if (rc != TPE_OK) return rc;
+  cudaStream_t st = ctx->stream;
+  CU(s.prm.ensure((size_t)k * (P + 2) * 8));
+  CU(s.beta.ensure(k * 8));
+  CU(s.Xs.ensure((size_t)ns * 8));
+  CU(s.out.ensure(k * 3 * 8));
+  CU(cudaMemcpyAsync(s.prm.p, params, (size_t)k * (P + 2) * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.beta.p, beta, k * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.Xs.p, samples, (size_t)ns * 8, cudaMemcpyHostToDevice, st));
+  gpb::k_gpb_bounds<<<(unsigned)k, gpb::THREADS, smem, st>>>(
+      s.X.as<double>(), s.y.as<double>(), s.doff.as<int64_t>(), s.cat.as<uint8_t>(), P, s.idx.as<int32_t>(),
+      s.prm.as<double>(), s.beta.as<double>(), s.Xs.as<double>(), S, s.ws.as<double>(), s.wsoff.as<int64_t>(),
+      s.out.as<double>(), s.status.as<int32_t>());
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(out, s.out.p, k * 3 * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(status, s.status.p, k * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
 static constexpr int64_t kEhviPartDoubles = (int64_t)1 << 23;   // partial sums of one launch at most (64 MB)
 
 // the chunk kernel for M objectives: register arrays sized for the next of 4, 8, 12, 24 (a 16 spills with gradients)

@@ -505,6 +505,56 @@ class TPEEngine:
                                            _ptr(dvar)))
         return (mean, var, dmean, dvar) if grad else (mean, var)
 
+    def gp_batch_set(self, offsets, X, y, is_categorical) -> None:
+        """Many independent GPs at once (tpe_gp_batch_set): GP i is fitted to the rows ``offsets[i] ..
+        offsets[i + 1] - 1`` of ``X`` [N, P] and ``y`` [N]; all share ``is_categorical`` [P].  ``ValueError`` on bad
+        input, or naming the bytes when the device lacks the memory.  Leaves the other state of this engine
+        unchanged."""
+        off = np.ascontiguousarray(offsets, dtype=np.int64)
+        Xa, ya = _f64(X), _f64(y)
+        cat = np.ascontiguousarray(is_categorical, dtype=np.uint8)
+        if off.ndim != 1 or Xa.ndim != 2 or ya.shape != (Xa.shape[0],) or cat.shape != (Xa.shape[1],) or (
+                off.size and off[-1] != Xa.shape[0]):
+            raise ValueError(f"batched GP data must be offsets [n_gp + 1] ending at N, X [N, P], y [N], "
+                             f"is_categorical [P]; got {off.shape}, {Xa.shape}, {ya.shape}, {cat.shape}")
+        self._gpb_P = 0   # a failed call leaves no batched GP data in the context either
+        self._check(self._lib.tpe_gp_batch_set(self._h, off.size - 1, _ptr(off), Xa.shape[1], _ptr(Xa), _ptr(ya),
+                                               _ptr(cat)))
+        self._gpb_P = Xa.shape[1]
+
+    def gp_batch_loss(self, gp_idx, raw, minimum_noise: float):
+        """``gp_loss`` for k jobs at once (tpe_gp_batch_loss): job b is GP ``gp_idx[b]`` at ``raw[b]`` [P + 2].
+        Returns ``(loss [k], grad [k, P + 2], status [k])``; status 1 marks a job whose covariance is not positive
+        definite (or whose kernel parameters are not finite), its loss and gradient NaN."""
+        idx = np.ascontiguousarray(gp_idx, dtype=np.int32)
+        r = _f64(raw)
+        P = getattr(self, "_gpb_P", 0)
+        if idx.ndim != 1 or (P and r.shape != (idx.size, P + 2)):
+            raise ValueError(f"raw must be [k, {P + 2}] for k = {idx.size} GP indices, got shape {r.shape}")
+        loss, grad = np.empty(idx.size), np.empty(r.shape)
+        status = np.empty(idx.size, dtype=np.int32)
+        self._check(self._lib.tpe_gp_batch_loss(self._h, idx.size, _ptr(idx), _ptr(r), float(minimum_noise),
+                                                _ptr(loss), _ptr(grad), _ptr(status)))
+        return loss, grad, status
+
+    def gp_batch_bounds(self, gp_idx, params, beta, samples):
+        """RegretBoundEvaluator's three maxima for k jobs (tpe_gp_batch_bounds): job b is GP ``gp_idx[b]`` at
+        ``params[b]`` [P + 2] (inverse squared lengthscales, kernel scale, noise_var) with ``beta[b]`` and the sample
+        rows ``samples[b]`` [S, P].  Returns ``(out [k, 3], status [k])``: max UCB over the train rows, max UCB over
+        the samples, max LCB over the train rows; status as for ``gp_batch_loss``."""
+        idx = np.ascontiguousarray(gp_idx, dtype=np.int32)
+        prm, bt, xs = _f64(params), _f64(beta), _f64(samples)
+        P = getattr(self, "_gpb_P", 0)
+        if idx.ndim != 1 or bt.shape != idx.shape or xs.ndim != 3 or xs.shape[0] != idx.size or (
+                P and (prm.shape != (idx.size, P + 2) or xs.shape[2] != P)):
+            raise ValueError(f"bounds need params [k, {P + 2}], beta [k], samples [k, S, {P}]; got {prm.shape}, "
+                             f"{bt.shape}, {xs.shape}")
+        out = np.empty((idx.size, 3))
+        status = np.empty(idx.size, dtype=np.int32)
+        self._check(self._lib.tpe_gp_batch_bounds(self._h, idx.size, _ptr(idx), _ptr(prm), _ptr(bt), xs.shape[1],
+                                                  _ptr(xs), _ptr(out), _ptr(status)))
+        return out, status
+
     def ehvi_set(self, lower, intervals, samples) -> None:
         """The non-dominated boxes and fixed QMC samples of a log-EHVI acquisition (tpe_ehvi_set): ``lower`` and
         ``intervals`` [B, M] (intervals already clamped at 1e-12), ``samples`` [S, M].  2 <= M <= 24, 1 <= S <= 1024,

@@ -19,8 +19,10 @@ host and cannot run at those sizes at all.
 """
 from __future__ import annotations
 
+import contextlib
 import math
 import sys
+import threading
 
 import numpy as np
 import scipy.stats
@@ -79,7 +81,8 @@ def _loss_and_grad(engine, raw_params: np.ndarray, n_params: int, log_prior, min
 
 
 def _fit_kernel_params(engine, n_params: int, log_prior, minimum_noise: float, initial_params: np.ndarray,
-                       deterministic_objective: bool = False, gtol: float = 1e-2) -> np.ndarray:
+                       deterministic_objective: bool = False, gtol: float = 1e-2,
+                       single_blas: bool = True) -> np.ndarray:
     """``GPRegressor._fit_kernel_params`` (gp.py:287-351) from ``initial_params`` = (inverse squared lengthscales,
     kernel scale, noise_var): returns the fitted parameters in the same form, as the GP stores them.  The negative
     marginal log-likelihood and its gradient come from the device, the prior term from ``log_prior`` with torch
@@ -95,7 +98,8 @@ def _fit_kernel_params(engine, n_params: int, log_prior, minimum_noise: float, i
     def loss_func(raw_params: np.ndarray) -> tuple[float, np.ndarray]:
         return _loss_and_grad(engine, raw_params, n_params, log_prior, minimum_noise, deterministic_objective)
 
-    with single_blas_thread_if_scipy_v1_15_or_newer():
+    # single_blas=False: the caller (the lock-step batch, which runs many fits in threads) holds the limit
+    with single_blas_thread_if_scipy_v1_15_or_newer() if single_blas else contextlib.nullcontext():
         res = scipy.optimize.minimize(loss_func, initial_raw_params, jac=True, method="l-bfgs-b",
                                       options={"gtol": gtol})
     if not res.success:
@@ -106,7 +110,7 @@ def _fit_kernel_params(engine, n_params: int, log_prior, minimum_noise: float, i
 
 
 def _fit(engine, n_params: int, log_prior, minimum_noise: float, gpr_cache: np.ndarray | None = None,
-         deterministic_objective: bool = False) -> np.ndarray:
+         deterministic_objective: bool = False, single_blas: bool = True) -> np.ndarray:
     """``fit_kernel_params`` (gp.py:354-409): a first attempt from ``gpr_cache`` (the parameters an earlier fit
     returned; the default parameters when None), a second from the default parameters, then the warning and the
     default GP, whose noise_var is 1 whatever ``deterministic_objective`` is."""
@@ -115,7 +119,7 @@ def _fit(engine, n_params: int, log_prior, minimum_noise: float, gpr_cache: np.n
     for initial_params in (default_params if gpr_cache is None else gpr_cache, default_params):
         try:
             return _fit_kernel_params(engine, n_params, log_prior, minimum_noise, initial_params,
-                                      deterministic_objective)
+                                      deterministic_objective, single_blas=single_blas)
         except RuntimeError as e:
             error = e
     _logger.warning(
@@ -315,3 +319,293 @@ class EMMREvaluator(_OptunaEMMREvaluator):
             + alg1_delta_r_tilde_t_term4,
         )
 
+
+
+# ---- the whole improvement curve at once ------------------------------------------------------------------------------
+# Upper bound on the device memory one wave of batched fits may take (data, workspace and sample rows).  A private
+# module constant so that tests can make every wave a single GP.
+_WAVE_BYTES = 4 << 30
+
+
+def _wave_bytes(n: int, P: int, n_samples: int) -> int:
+    """Device bytes one GP of n rows adds to a wave: its rows, the workspace of tpe_gpbatch.cuh (an n x n matrix and
+    three n-vectors above 160 rows, and n x 256 doubles of cross covariance for the bounds) and its samples."""
+    ws = (n * n + 3 * n if n > 160 else 0) + n * 256
+    return 8 * (n * (P + 1) + ws + n_samples * P + 2 * (P + 2) + 8)
+
+
+class _Prefix:
+    """What ``RegretBoundEvaluator.evaluate`` forms for one trial prefix before its fit (evaluator.py:142-163)."""
+
+    __slots__ = ("X", "y", "std", "is_categorical", "beta", "samples", "gp", "failed")
+
+
+class _LockStep:
+    """Lock-step L-BFGS-B: one scipy fit per GP in its own thread.  A thread's loss call posts its raw parameters and
+    blocks; ``run`` evaluates everything posted in one ``gp_batch_loss``, then releases the threads one at a time and
+    waits for each to post again or finish.  So one fit thread runs at a time (the host work is serial under the GIL
+    anyway) and the threads do not contend for the GIL; a thread whose fit has returned leaves the batch."""
+
+    def __init__(self, engine, minimum_noise: float) -> None:
+        self._engine = engine
+        self._minimum_noise = minimum_noise
+        self._cond = threading.Condition()
+        self._posted: dict[int, np.ndarray] = {}
+        self._left: set[int] = set()
+        self._results: dict[int, tuple] = {}
+        self._events: dict[int, threading.Event] = {}
+        self.rounds = 0
+        self.device_seconds = 0.0
+
+    def slot(self, gp: int) -> "_Slot":
+        self._events[gp] = threading.Event()
+        return _Slot(self, gp)
+
+    def post(self, gp: int, raw: np.ndarray):
+        ev = self._events[gp]
+        with self._cond:
+            self._posted[gp] = raw
+            self._cond.notify()
+        ev.wait()
+        ev.clear()
+        return self._results.pop(gp)
+
+    def leave(self, gp: int) -> None:
+        with self._cond:
+            self._left.add(gp)
+            self._cond.notify()
+
+    def _wait(self, gp: int) -> None:
+        with self._cond:
+            while gp not in self._posted and gp not in self._left:
+                self._cond.wait()
+
+    def run(self, threads: list) -> None:
+        import time
+        for gp, th in enumerate(threads):
+            th.start()
+            self._wait(gp)
+        while self._posted:
+            batch, self._posted = self._posted, {}
+            gps = sorted(batch)
+            t0 = time.perf_counter()
+            loss, grad, status = self._engine.gp_batch_loss(gps, np.stack([batch[g] for g in gps]),
+                                                            self._minimum_noise)
+            self.device_seconds += time.perf_counter() - t0
+            self.rounds += 1
+            for i, g in enumerate(gps):
+                self._results[g] = (float(loss[i]), grad[i].copy(), int(status[i]))
+                self._events[g].set()
+                self._wait(g)
+
+
+class _Slot:
+    """The engine a fit thread sees: ``gp_loss`` answered by the lock-step batch."""
+
+    def __init__(self, lockstep: _LockStep, gp: int) -> None:
+        self._ls = lockstep
+        self._gp = gp
+
+    def gp_loss(self, raw_params, minimum_noise: float):
+        loss, grad, status = self._ls.post(self._gp, np.array(raw_params, dtype=np.float64))
+        if status:
+            raise GPCholeskyError("the GP covariance is not positive definite")
+        return loss, grad
+
+
+def _prepare_prefixes(evaluator: "RegretBoundEvaluator", study) -> tuple[list[int], list[_Prefix]]:
+    """The host pre-pass, in the reference's trial order: per prefix the data of ``evaluate`` and its 2048 samples
+    from the evaluator's own stream.  Prefixes whose complete trials are the same share one GP."""
+    trial_numbers: list[int] = []
+    prefixes: list[_Prefix] = []
+    completed: list[FrozenTrial] = []
+    last: _Prefix | None = None
+    last_n = -1
+    rng = evaluator._rng.rng
+    direction = study.direction
+    for trial in study.trials:
+        if trial.state == TrialState.COMPLETE:
+            completed.append(trial)
+        if not completed:
+            continue
+        trial_numbers.append(trial.number)
+        p = _Prefix()
+        if len(completed) == last_n:
+            p.X, p.y, p.std, p.is_categorical, p.beta = last.X, last.y, last.std, last.is_categorical, last.beta
+            space = last_space
+        else:
+            trials = list(completed)
+            optuna_search_space = intersection_search_space(trials)
+            evaluator._validate_input(trials, optuna_search_space)
+            sign = -1 if direction == StudyDirection.MINIMIZE else 1
+            values = np.array([t.value for t in trials]) * sign
+            space = gp_search_space.SearchSpace(optuna_search_space)
+            normalized_params = space.get_normalized_params(trials)
+            p.X, top_n_values = evaluator._get_top_n(normalized_params, values)
+            top_n_values_mean = top_n_values.mean()
+            p.std = max(1e-10, top_n_values.std())
+            p.y = (top_n_values - top_n_values_mean) / p.std
+            p.is_categorical = space.is_categorical
+            p.beta = _get_beta(p.X.shape[1], p.X.shape[0])
+        p.samples = space.sample_normalized_params(evaluator._optimize_n_samples, rng=rng)
+        p.failed = False
+        prefixes.append(p)
+        last, last_n, last_space = p, len(completed), space
+    return trial_numbers, prefixes
+
+
+def _batched_improvements(evaluator: "RegretBoundEvaluator", study, stats: dict | None = None) -> tuple[list, list]:
+    import time
+    rng = evaluator._rng.rng
+    start_state = rng.get_state()
+    trial_numbers, prefixes = _prepare_prefixes(evaluator, study)
+    if not prefixes:
+        return [], []
+    # the distinct GPs (one per distinct complete set), grouped by P, in waves bounded by _WAVE_BYTES
+    gps: list[_Prefix] = []
+    for p in prefixes:
+        if not gps or p.X is not gps[-1].X:
+            gps.append(p)
+        p.gp = len(gps) - 1
+    by_p: dict[int, list[int]] = {}
+    for i, g in enumerate(gps):
+        by_p.setdefault(g.X.shape[1], []).append(i)
+    params: list[np.ndarray | None] = [None] * len(gps)
+    n_samples = evaluator._optimize_n_samples
+    out = np.empty((len(prefixes), 3))
+    users = [[] for _ in gps]
+    for j, p in enumerate(prefixes):
+        users[p.gp].append(j)
+    engine = _engine_cls(evaluator._device)
+    t_all = time.perf_counter()
+    try:
+        with single_blas_thread_if_scipy_v1_15_or_newer():
+            for P, members in by_p.items():
+                waves: list[list[int]] = [[]]
+                used = 0
+                for i in members:
+                    need = _wave_bytes(gps[i].X.shape[0], P, n_samples * len(users[i]))
+                    if waves[-1] and used + need > _WAVE_BYTES:
+                        waves.append([])
+                        used = 0
+                    waves[-1].append(i)
+                    used += need
+                for wave in waves:
+                    _run_wave(engine, evaluator, gps, wave, users, prefixes, params, out, stats)
+    finally:
+        engine.close()
+    if stats is not None:
+        stats["wall_seconds"] = time.perf_counter() - t_all
+    # the reference raises at the first prefix whose final covariance is not positive definite, after drawing that
+    # prefix's samples: leave the stream there
+    for j, p in enumerate(prefixes):
+        if p.failed:
+            rng.set_state(start_state)
+            _prepare_prefixes_upto(evaluator, study, j)
+            raise np.linalg.LinAlgError("Matrix is not positive definite")
+    improvements = []
+    for j, p in enumerate(prefixes):
+        standardized_ucb_value = max(out[j, 0], out[j, 1])
+        standardized_lcb_value = out[j, 2]
+        improvements.append((standardized_ucb_value - standardized_lcb_value) * p.std)
+    return trial_numbers, improvements
+
+
+def _prepare_prefixes_upto(evaluator, study, last: int) -> None:
+    """Redraws the samples of the prefixes 0 .. last, so that the stream is where the reference leaves it when it
+    raises at prefix ``last``."""
+    rng = evaluator._rng.rng
+    completed = []
+    j = -1
+    space = None
+    last_n = -1
+    for trial in study.trials:
+        if trial.state == TrialState.COMPLETE:
+            completed.append(trial)
+        if not completed:
+            continue
+        j += 1
+        if len(completed) != last_n:
+            space = gp_search_space.SearchSpace(intersection_search_space(list(completed)))
+            last_n = len(completed)
+        space.sample_normalized_params(evaluator._optimize_n_samples, rng=rng)
+        if j == last:
+            return
+
+
+def _run_wave(engine, evaluator, gps, wave, users, prefixes, params, out, stats) -> None:
+    """Fits the GPs of one wave in lock step, then the bounds of every prefix that uses them."""
+    P = gps[wave[0]].X.shape[1]
+    offsets = np.zeros(len(wave) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([gps[i].X.shape[0] for i in wave])
+    engine.gp_batch_set(offsets, np.concatenate([gps[i].X for i in wave]), np.concatenate([gps[i].y for i in wave]),
+                        gps[wave[0]].is_categorical)
+    ls = _LockStep(engine, evaluator._minimum_noise)
+    results: dict[int, np.ndarray] = {}
+    errors: dict[int, BaseException] = {}
+
+    def work(local: int, slot: _Slot) -> None:
+        try:
+            results[local] = _fit(slot, P, evaluator._log_prior, evaluator._minimum_noise, single_blas=False)
+        except BaseException as e:   # re-raised below, in prefix order
+            errors[local] = e
+        finally:
+            ls.leave(local)
+
+    threads = [threading.Thread(target=work, args=(k, ls.slot(k)), daemon=True) for k in range(len(wave))]
+    ls.run(threads)
+    for th in threads:
+        th.join()
+    if errors:
+        raise errors[min(errors)]
+    if stats is not None:
+        stats["rounds"] = stats.get("rounds", 0) + ls.rounds
+        stats["device_seconds"] = stats.get("device_seconds", 0.0) + ls.device_seconds
+    jobs = [(k, j) for k, i in enumerate(wave) for j in users[i]]
+    idx = np.array([k for k, _ in jobs], dtype=np.int32)
+    prm = np.stack([results[k] for k, _ in jobs])
+    beta = np.array([prefixes[j].beta for _, j in jobs])
+    samples = np.stack([prefixes[j].samples for _, j in jobs])
+    res, status = engine.gp_batch_bounds(idx, prm, beta, samples)
+    for r, (k, j), st in zip(res, jobs, status):
+        out[j] = r
+        prefixes[j].failed = bool(st)
+
+
+def terminator_improvement_history(study, improvement_evaluator=None, error_evaluator=None, get_error: bool = False):
+    """The terminator's improvement after every trial of ``study``: what
+    ``optuna.visualization._terminator_improvement._get_improvement_info`` returns, with the same trial walk, the
+    same arguments and the same errors.
+
+    With the default evaluator, or an evaluator whose type is exactly ``optuna_b200.RegretBoundEvaluator``, the
+    Gaussian processes of every trial prefix are fitted together: the host forms each prefix's data and draws its
+    samples from the evaluator's stream in the reference's order, then one device launch per L-BFGS-B round
+    evaluates every live fit (``tpe_gp_batch_loss``) and one more gives every prefix's bounds.  Any other improvement
+    evaluator takes optuna's per-prefix loop unchanged.  Error evaluators are called per prefix, as the reference
+    calls them."""
+    from optuna.terminator import CrossValidationErrorEvaluator, StaticErrorEvaluator
+    from optuna.terminator.improvement.evaluator import BestValueStagnationEvaluator
+    from optuna.visualization._terminator_improvement import _get_improvement_info, _ImprovementInfo
+
+    if study._is_multi_objective():
+        raise ValueError("This function does not support multi-objective optimization study.")
+    if improvement_evaluator is None:
+        improvement_evaluator = RegretBoundEvaluator()
+    if error_evaluator is None:
+        if isinstance(improvement_evaluator, BestValueStagnationEvaluator):
+            error_evaluator = StaticErrorEvaluator(constant=0)
+        else:
+            error_evaluator = CrossValidationErrorEvaluator()
+    if type(improvement_evaluator) is not RegretBoundEvaluator:
+        return _get_improvement_info(study, get_error, improvement_evaluator, error_evaluator)
+    trial_numbers, improvements = _batched_improvements(improvement_evaluator, study)
+    errors = []
+    if get_error:
+        completed: list[FrozenTrial] = []
+        for trial in study.trials:
+            if trial.state == TrialState.COMPLETE:
+                completed.append(trial)
+            if not completed:
+                continue
+            errors.append(error_evaluator.evaluate(trials=completed, study_direction=study.direction))
+    return _ImprovementInfo(trial_numbers=trial_numbers, improvements=improvements, errors=errors or None)
