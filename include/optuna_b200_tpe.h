@@ -44,7 +44,8 @@ extern "C" {
 /* 13: + tpe_ehvi_set, tpe_ehvi */
 /* 14: + tpe_box_decomposition, tpe_get_box_decomposition */
 /* 15: + tpe_gp_batch_set, tpe_gp_batch_loss, tpe_gp_batch_bounds */
-#define TPE_ABI_VERSION 15
+/* 16: + tpe_gp_batch_loss_fixed_noise, tpe_gp_batch_moments */
+#define TPE_ABI_VERSION 16
 
 enum {
   TPE_OK = 0,
@@ -353,6 +354,14 @@ int tpe_gp_query(tpe_ctx* ctx, const double* Xq, int64_t m, double* mean, double
  * mean + sqrt(beta var), the same over the sample rows, and max over the train rows of mean - sqrt(beta var), var
  * clamped at 0 and NaN propagating as np.max propagates it (RegretBoundEvaluator.evaluate, optuna/terminator/
  * improvement/evaluator.py:50-84).  status as for the loss.
+ * tpe_gp_batch_loss_fixed_noise is tpe_gp_loss_fixed_noise for k jobs: the noise is fixed at noise_var, raw[b][P + 1]
+ * is not read and grad[b][P + 1] = 0; status as for tpe_gp_batch_loss.
+ * tpe_gp_batch_moments replaces the posterior calls of EMMREvaluator.evaluate (optuna/terminator/improvement/emmr.py:
+ * 165-185) for k jobs: job b is GP gp_idx[b] at params[b] [P + 2] (inverse squared lengthscales, kernel scale,
+ * noise_var), queried at m (1 to 3) of its own train rows, rows[b] [m] row indices within the GP.  mean[b] [m] and
+ * var[b] [m] clamped at 0; with n_joint in [2, m] also cov[b] [n_joint * n_joint] row-major, the joint covariance of
+ * the first n_joint rows with its diagonal clamped at 0 (tpe_gp_posterior_moments's); n_joint = 0 and cov = NULL for
+ * none.  status as for the loss, with the outputs NaN.  TPE_E_INVALID for a row index outside its GP or a bad n_joint.
  * Several jobs may name the same GP.  A job's outputs are the same bits whatever the other jobs of the call are. */
 int tpe_gp_batch_set(tpe_ctx* ctx, int32_t n_gp, const int64_t* offsets, int32_t P, const double* X, const double* y,
                      const uint8_t* is_categorical);
@@ -360,6 +369,11 @@ int tpe_gp_batch_loss(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const doub
                       double* loss, double* grad, int32_t* status);
 int tpe_gp_batch_bounds(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* params, const double* beta,
                         int32_t S, const double* samples, double* out, int32_t* status);
+int tpe_gp_batch_loss_fixed_noise(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* raw, double noise_var,
+                                  double* loss, double* grad, int32_t* status);
+int tpe_gp_batch_moments(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* params, int32_t m,
+                         const int32_t* rows, int32_t n_joint, double* mean, double* var, double* cov,
+                         int32_t* status);
 /* Log expected hypervolume improvement of GPSampler's multi-objective acquisition (LogEHVI, optuna/_gp/acqf.py:245-300,
  * with logehvi :45-62), fp64.  Kept apart from the history, the suggestion state and the GP state.
  * tpe_ehvi_set replaces the state LogEHVI.__init__ builds (acqf.py:245-280): lower [B, M] the lower bounds of the

@@ -88,6 +88,8 @@ SYMBOLS = {
     "tpe_gp_batch_set": (C.c_int, [_P, C.c_int32, _P, C.c_int32, _P, _P, _P]),
     "tpe_gp_batch_loss": (C.c_int, [_P, C.c_int64, _P, _P, C.c_double, _P, _P, _P]),
     "tpe_gp_batch_bounds": (C.c_int, [_P, C.c_int64, _P, _P, _P, C.c_int32, _P, _P, _P]),
+    "tpe_gp_batch_loss_fixed_noise": (C.c_int, [_P, C.c_int64, _P, _P, C.c_double, _P, _P, _P]),
+    "tpe_gp_batch_moments": (C.c_int, [_P, C.c_int64, _P, _P, C.c_int32, _P, C.c_int32, _P, _P, _P, _P]),
     "tpe_get_candidates": (C.c_int, [_P, _P, _P, _P]),
     "tpe_logpdf": (C.c_int, [_P, C.c_int, _P, C.c_int64, _P]),
     "tpe_last_timing": (C.c_int, [_P, _P, _P]),
@@ -98,7 +100,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 15  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 16  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

@@ -253,9 +253,9 @@ def plot_pareto_front(study, *, target_names: list[str] | None = None, include_d
 def plot_terminator_improvement(study, plot_error: bool = False, improvement_evaluator=None, error_evaluator=None,
                                 min_n_trials: int = 20):
     """Drop-in for ``optuna.visualization.plot_terminator_improvement``: the same ``plotly`` figure, with the
-    improvement of every trial prefix from ``optuna_b200.terminator_improvement_history`` (all prefixes' Gaussian
-    processes fitted together on the GPU for ``optuna_b200.RegretBoundEvaluator``, the default).  Needs plotly, as
-    optuna's does."""
+    improvement of every trial prefix from ``optuna_b200.terminator_improvement_history``: all prefixes' Gaussian
+    processes are fitted together on the GPU for ``optuna_b200.RegretBoundEvaluator`` (the default), and both
+    Gaussian processes of every prefix for ``optuna_b200.EMMREvaluator``.  Needs plotly, as optuna's does."""
     from optuna.visualization._plotly_imports import _imports
     from optuna.visualization._terminator_improvement import _get_improvement_plot
 

@@ -24,6 +24,7 @@
 #include "tpe_fanova.cuh"
 #include "tpe_gp.cuh"
 #include "tpe_gpbatch.cuh"
+#include "tpe_gpemmr.cuh"
 #include "tpe_ehvi.cuh"
 #include "tpe_boxdec.cuh"
 #include "tpe_uni.cuh"
@@ -143,10 +144,11 @@ struct GpState {
 struct GpBatchState {
   int32_t n_gp = 0, P = 0;
   std::vector<int64_t> off;   // host copy of the row offsets [n_gp + 1]
-  DevBuf X, y, doff, cat, idx, prm, nexc, ws, wsoff, loss, grad, status, beta, Xs, out;
+  DevBuf X, y, doff, cat, idx, prm, nexc, ws, wsoff, loss, grad, status, beta, Xs, out, rows;
   bool ready = false;
   void release() {
-    for (DevBuf* b : {&X, &y, &doff, &cat, &idx, &prm, &nexc, &ws, &wsoff, &loss, &grad, &status, &beta, &Xs, &out})
+    for (DevBuf* b : {&X, &y, &doff, &cat, &idx, &prm, &nexc, &ws, &wsoff, &loss, &grad, &status, &beta, &Xs, &out,
+                      &rows})
       b->release();
     *this = GpBatchState();
   }
@@ -4149,9 +4151,13 @@ static size_t gpb_free_bytes(tpe_ctx* ctx) {
   return free_b;
 }
 
+// The three kinds of batched call, by the per-job workspace they need
+enum GpbCall { GPB_LOSS, GPB_BOUNDS, GPB_MOMENTS };
+
 // Per-job workspace offsets (doubles) of a call: k_gpb_loss needs gpb::ws_doubles(n), k_gpb_bounds also n x NQ
-// doubles of cross covariance.  Jobs get their own workspace even when they name the same GP.
-static int64_t gpb_ws_layout(const GpBatchState& s, const int32_t* gp_idx, int64_t k, bool bounds,
+// doubles of cross covariance, k_gpe_moments gpe::ws_doubles(n).  Jobs get their own workspace even when they name the
+// same GP.
+static int64_t gpb_ws_layout(const GpBatchState& s, const int32_t* gp_idx, int64_t k, GpbCall call,
                              std::vector<int64_t>& wsoff, size_t* smem) {
   int64_t tot = 0;
   *smem = 0;
@@ -4159,7 +4165,7 @@ static int64_t gpb_ws_layout(const GpBatchState& s, const int32_t* gp_idx, int64
   for (int64_t b = 0; b < k; ++b) {
     const int64_t n = s.off[gp_idx[b] + 1] - s.off[gp_idx[b]];
     wsoff[b] = tot;
-    tot += gpb::ws_doubles(n) + (bounds ? n * gpb::NQ : 0);
+    tot += call == GPB_MOMENTS ? gpe::ws_doubles(n) : gpb::ws_doubles(n) + (call == GPB_BOUNDS ? n * gpb::NQ : 0);
     *smem = std::max(*smem, gpb::smem_bytes((int)n, s.P));
   }
   return tot;
@@ -4183,17 +4189,20 @@ static int gpb_oom(tpe_ctx* ctx, const char* what, size_t need, int64_t nmax) {
 
 // Uploads the job list and sizes the per-job workspace and the launch's shared memory; the caller has checked the
 // jobs.  Fails naming the bytes when the workspace does not fit in free device memory.
-static int gpb_stage_jobs(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, bool bounds, size_t extra,
+static int gpb_stage_jobs(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, GpbCall call, size_t extra,
                           size_t* smem) {
   GpBatchState& s = ctx->gpb;
   std::vector<int64_t> wsoff;
-  const int64_t wsd = gpb_ws_layout(s, gp_idx, k, bounds, wsoff, smem);
+  const int64_t wsd = gpb_ws_layout(s, gp_idx, k, call, wsoff, smem);
   int64_t nmax = 0;
   for (int64_t b = 0; b < k; ++b) nmax = std::max(nmax, s.off[gp_idx[b] + 1] - s.off[gp_idx[b]]);
   const size_t need = (size_t)std::max<int64_t>(wsd, 1) * 8 + extra;
   const size_t have = s.ws.cap;
   if (need > have && need - have > gpb_free_bytes(ctx))
-    return gpb_oom(ctx, bounds ? "the batched GP bounds" : "the batched GP loss", need, nmax);
+    return gpb_oom(ctx,
+                   call == GPB_BOUNDS ? "the batched GP bounds"
+                                      : call == GPB_MOMENTS ? "the batched GP moments" : "the batched GP loss",
+                   need, nmax);
   cudaStream_t st = ctx->stream;
   CU(s.ws.ensure((size_t)std::max<int64_t>(wsd, 1) * 8));
   CU(s.wsoff.ensure(k * 8));
@@ -4204,6 +4213,7 @@ static int gpb_stage_jobs(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, bool b
   if (*smem > 48 * 1024) {
     CU(cudaFuncSetAttribute(gpb::k_gpb_loss, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
     CU(cudaFuncSetAttribute(gpb::k_gpb_bounds, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
+    CU(cudaFuncSetAttribute(gpe::k_gpe_moments, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)*smem));
   }
   return TPE_OK;
 }
@@ -4256,20 +4266,21 @@ int tpe_gp_batch_set(tpe_ctx* ctx, int32_t n_gp, const int64_t* offsets, int32_t
   return TPE_OK;
 }
 
-// tpe_gp_loss for k jobs at once: job b is GP gp_idx[b] at raw[b] [P + 2]
-int tpe_gp_batch_loss(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* raw, double minimum_noise,
-                      double* loss, double* grad, int32_t* status) {
-  if (!ctx) return TPE_E_INVALID;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+// The body of tpe_gp_batch_loss and tpe_gp_batch_loss_fixed_noise, called under the context lock: job b's noise is
+// exp(raw[b][P + 1]) + noise, or with fixed the constant noise with a noise excess of 0, which makes k_gpb_loss's raw
+// noise gradient 1/2 * 0 * sum_i W_ii = 0 (k_gp_grad_tail's form, as tpe_gp_loss_fixed_noise gives it)
+static int gpb_loss_run(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* raw, double noise, bool fixed,
+                        double* loss, double* grad, int32_t* status) {
   int rc = gpb_check_jobs(ctx, k, gp_idx);
   if (rc != TPE_OK) return rc;
   if (!raw || !loss || !grad || !status) return fail(ctx, TPE_E_INVALID, "bad batched GP loss arguments");
-  if (!std::isfinite(minimum_noise) || minimum_noise < 0.0) return fail(ctx, TPE_E_INVALID, "bad minimum noise");
+  if (!std::isfinite(noise) || noise < 0.0)
+    return fail(ctx, TPE_E_INVALID, fixed ? "bad noise variance" : "bad minimum noise");
   GpBatchState& s = ctx->gpb;
   const int P = s.P;
   if (set_device(ctx)) return TPE_E_CUDA;
   size_t smem = 0;
-  rc = gpb_stage_jobs(ctx, k, gp_idx, false, 0, &smem);
+  rc = gpb_stage_jobs(ctx, k, gp_idx, GPB_LOSS, 0, &smem);
   if (rc != TPE_OK) return rc;
   // the kernel parameters as tpe_gp_loss forms them on the host; a non-finite one is reported by the kernel
   std::vector<double> prm((size_t)k * (P + 2)), nexc(k);
@@ -4277,8 +4288,8 @@ int tpe_gp_batch_loss(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const doub
     const double* r = raw + b * (P + 2);
     double* p = prm.data() + b * (P + 2);
     for (int d = 0; d <= P; ++d) p[d] = std::exp(r[d]);
-    nexc[b] = std::exp(r[P + 1]);
-    p[P + 1] = nexc[b] + minimum_noise;
+    nexc[b] = fixed ? 0.0 : std::exp(r[P + 1]);
+    p[P + 1] = nexc[b] + noise;
   }
   cudaStream_t st = ctx->stream;
   CU(s.prm.ensure(prm.size() * 8));
@@ -4297,6 +4308,22 @@ int tpe_gp_batch_loss(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const doub
   CU(cudaMemcpyAsync(status, s.status.p, k * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return TPE_OK;
+}
+
+// tpe_gp_loss for k jobs at once: job b is GP gp_idx[b] at raw[b] [P + 2]
+int tpe_gp_batch_loss(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* raw, double minimum_noise,
+                      double* loss, double* grad, int32_t* status) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  return gpb_loss_run(ctx, k, gp_idx, raw, minimum_noise, false, loss, grad, status);
+}
+
+// tpe_gp_loss_fixed_noise for k jobs at once: the noise is noise_var, raw[b][P + 1] is not read, grad[b][P + 1] = 0
+int tpe_gp_batch_loss_fixed_noise(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* raw, double noise_var,
+                                  double* loss, double* grad, int32_t* status) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  return gpb_loss_run(ctx, k, gp_idx, raw, noise_var, true, loss, grad, status);
 }
 
 // RegretBoundEvaluator's three maxima for k jobs: GP gp_idx[b] at params[b] [P + 2], beta[b], and its S sample rows
@@ -4318,7 +4345,7 @@ int tpe_gp_batch_bounds(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const do
     if (!std::isfinite(samples[i])) return fail(ctx, TPE_E_INVALID, "sample points hold a non-finite value");
   if (set_device(ctx)) return TPE_E_CUDA;
   size_t smem = 0;
-  rc = gpb_stage_jobs(ctx, k, gp_idx, true, (size_t)ns * 8, &smem);
+  rc = gpb_stage_jobs(ctx, k, gp_idx, GPB_BOUNDS, (size_t)ns * 8, &smem);
   if (rc != TPE_OK) return rc;
   cudaStream_t st = ctx->stream;
   CU(s.prm.ensure((size_t)k * (P + 2) * 8));
@@ -4334,6 +4361,56 @@ int tpe_gp_batch_bounds(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const do
       s.out.as<double>(), s.status.as<int32_t>());
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(out, s.out.p, k * 3 * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(status, s.status.p, k * 4, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
+// EMMREvaluator's posterior terms for k jobs: GP gp_idx[b] at params[b] [P + 2], at its own train rows rows[b] [m]
+int tpe_gp_batch_moments(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const double* params, int32_t m,
+                         const int32_t* rows, int32_t n_joint, double* mean, double* var, double* cov,
+                         int32_t* status) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  int rc = gpb_check_jobs(ctx, k, gp_idx);
+  if (rc != TPE_OK) return rc;
+  if (!params || !rows || !mean || !var || !status)
+    return fail(ctx, TPE_E_INVALID, "bad batched GP moments arguments");
+  if (m < 1 || m > gpe::MQ)
+    return fail(ctx, TPE_E_INVALID, "batched GP moments take 1 .. %d rows per job, got m = %d", gpe::MQ, m);
+  if (!(n_joint == 0 ? cov == nullptr : (n_joint >= 2 && n_joint <= m && cov != nullptr)))
+    return fail(ctx, TPE_E_INVALID, "bad joint covariance request (n_joint %d, m %d)", n_joint, m);
+  GpBatchState& s = ctx->gpb;
+  const int P = s.P;
+  for (int64_t b = 0; b < k; ++b) {
+    const int64_t n = s.off[gp_idx[b] + 1] - s.off[gp_idx[b]];
+    for (int q = 0; q < m; ++q)
+      if (rows[b * m + q] < 0 || rows[b * m + q] >= n)
+        return fail(ctx, TPE_E_INVALID, "row index %d of job %lld out of range (GP %d has %lld rows)", rows[b * m + q],
+                    (long long)b, gp_idx[b], (long long)n);
+  }
+  if (set_device(ctx)) return TPE_E_CUDA;
+  size_t smem = 0;
+  rc = gpb_stage_jobs(ctx, k, gp_idx, GPB_MOMENTS, 0, &smem);
+  if (rc != TPE_OK) return rc;
+  cudaStream_t st = ctx->stream;
+  const int64_t J2 = (int64_t)n_joint * n_joint;
+  CU(s.prm.ensure((size_t)k * (P + 2) * 8));
+  CU(s.rows.ensure((size_t)k * m * 4));
+  CU(s.out.ensure((size_t)k * (2 * m + J2) * 8));
+  double* dmean = s.out.as<double>();
+  double* dvar = dmean + k * m;
+  double* dcov = dvar + k * m;
+  CU(cudaMemcpyAsync(s.prm.p, params, (size_t)k * (P + 2) * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(s.rows.p, rows, (size_t)k * m * 4, cudaMemcpyHostToDevice, st));
+  gpe::k_gpe_moments<<<(unsigned)k, gpe::THREADS, smem, st>>>(
+      s.X.as<double>(), s.y.as<double>(), s.doff.as<int64_t>(), s.cat.as<uint8_t>(), P, s.idx.as<int32_t>(),
+      s.prm.as<double>(), s.rows.as<int32_t>(), m, n_joint, s.ws.as<double>(), s.wsoff.as<int64_t>(), dmean, dvar,
+      dcov, s.status.as<int32_t>());
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(mean, dmean, (size_t)k * m * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(var, dvar, (size_t)k * m * 8, cudaMemcpyDeviceToHost, st));
+  if (n_joint) CU(cudaMemcpyAsync(cov, dcov, (size_t)k * J2 * 8, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(status, s.status.p, k * 4, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
   return TPE_OK;

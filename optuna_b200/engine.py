@@ -522,10 +522,12 @@ class TPEEngine:
                                                _ptr(cat)))
         self._gpb_P = Xa.shape[1]
 
-    def gp_batch_loss(self, gp_idx, raw, minimum_noise: float):
+    def gp_batch_loss(self, gp_idx, raw, minimum_noise: float, deterministic: bool = False):
         """``gp_loss`` for k jobs at once (tpe_gp_batch_loss): job b is GP ``gp_idx[b]`` at ``raw[b]`` [P + 2].
         Returns ``(loss [k], grad [k, P + 2], status [k])``; status 1 marks a job whose covariance is not positive
-        definite (or whose kernel parameters are not finite), its loss and gradient NaN."""
+        definite (or whose kernel parameters are not finite), its loss and gradient NaN.  With ``deterministic`` the
+        noise is fixed at ``minimum_noise``, the last raw parameter is ignored and its gradient is 0
+        (tpe_gp_batch_loss_fixed_noise)."""
         idx = np.ascontiguousarray(gp_idx, dtype=np.int32)
         r = _f64(raw)
         P = getattr(self, "_gpb_P", 0)
@@ -533,8 +535,9 @@ class TPEEngine:
             raise ValueError(f"raw must be [k, {P + 2}] for k = {idx.size} GP indices, got shape {r.shape}")
         loss, grad = np.empty(idx.size), np.empty(r.shape)
         status = np.empty(idx.size, dtype=np.int32)
-        self._check(self._lib.tpe_gp_batch_loss(self._h, idx.size, _ptr(idx), _ptr(r), float(minimum_noise),
-                                                _ptr(loss), _ptr(grad), _ptr(status)))
+        fn = self._lib.tpe_gp_batch_loss_fixed_noise if deterministic else self._lib.tpe_gp_batch_loss
+        self._check(fn(self._h, idx.size, _ptr(idx), _ptr(r), float(minimum_noise), _ptr(loss), _ptr(grad),
+                       _ptr(status)))
         return loss, grad, status
 
     def gp_batch_bounds(self, gp_idx, params, beta, samples):
@@ -554,6 +557,29 @@ class TPEEngine:
         self._check(self._lib.tpe_gp_batch_bounds(self._h, idx.size, _ptr(idx), _ptr(prm), _ptr(bt), xs.shape[1],
                                                   _ptr(xs), _ptr(out), _ptr(status)))
         return out, status
+
+    def gp_batch_moments(self, gp_idx, params, rows, n_joint: int = 0):
+        """EMMREvaluator's posterior terms for k jobs (tpe_gp_batch_moments): job b is GP ``gp_idx[b]`` at
+        ``params[b]`` [P + 2] (inverse squared lengthscales, kernel scale, noise_var), queried at its own train rows
+        ``rows[b]`` [m] (row indices within the GP, 1 <= m <= 3).  Returns ``(mean [k, m], var [k, m], cov [k, J, J],
+        status [k])``: ``var`` clamped at 0, ``cov`` the joint covariance of the first ``J = n_joint`` rows (0, or 2
+        to m), diagonal clamped at 0; status as for ``gp_batch_loss``."""
+        idx = np.ascontiguousarray(gp_idx, dtype=np.int32)
+        prm = _f64(params)
+        rw = np.ascontiguousarray(rows, dtype=np.int32)
+        P = getattr(self, "_gpb_P", 0)
+        if idx.ndim != 1 or rw.ndim != 2 or rw.shape[0] != idx.size or (P and prm.shape != (idx.size, P + 2)):
+            raise ValueError(f"moments need params [k, {P + 2}] and rows [k, m]; got {prm.shape}, {rw.shape}")
+        n_joint = int(n_joint)
+        m = rw.shape[1]
+        mean, var = np.empty((idx.size, m)), np.empty((idx.size, m))
+        J = max(n_joint, 0)
+        cov = np.empty((idx.size, J, J))
+        status = np.empty(idx.size, dtype=np.int32)
+        self._check(self._lib.tpe_gp_batch_moments(self._h, idx.size, _ptr(idx), _ptr(prm), m, _ptr(rw), n_joint,
+                                                   _ptr(mean), _ptr(var), _ptr(cov) if n_joint else None,
+                                                   _ptr(status)))
+        return mean, var, cov, status
 
     def ehvi_set(self, lower, intervals, samples) -> None:
         """The non-dominated boxes and fixed QMC samples of a log-EHVI acquisition (tpe_ehvi_set): ``lower`` and

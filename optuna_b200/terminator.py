@@ -280,45 +280,51 @@ class EMMREvaluator(_OptunaEMMREvaluator):
         # emmr.py:249-250: for one point the reference takes the variance of the non-joint posterior
         cov_t_between_theta_t_star_and_theta_t1_star = float(
             var_t[0] if theta_t_star_index == theta_t1_star_index else cov_t[0, 1])
-        mu_t_theta_t_star, variance_t_theta_t_star = float(mean_t[0]), float(var_t[0])
-        variance_t_theta_t1_star = float(var_t[1])
-        mu_t1_theta_t_with_nu_t, variance_t1_theta_t_with_nu_t = float(mean_t[2]), float(var_t[2])
-        y_t = standarized_score_vals[-1]
+        return _emmr_criterion(kappa_t1, mu_t1_theta_t1_star, mean_t, var_t,
+                               cov_t_between_theta_t_star_and_theta_t1_star, standarized_score_vals[-1])
 
-        # emmr.py:198-237
-        theorem1_delta_mu_t_star = mu_t1_theta_t1_star - mu_t_theta_t_star
-        alg1_delta_r_tilde_t_term1 = theorem1_delta_mu_t_star
-        theorem1_v = math.sqrt(
-            max(
-                1e-10,
-                variance_t_theta_t_star
-                - 2.0 * cov_t_between_theta_t_star_and_theta_t1_star
-                + variance_t_theta_t1_star,
-            )
+
+def _emmr_criterion(kappa_t1: float, mu_t1_theta_t1_star: float, mean_t, var_t,
+                    cov_t_between_theta_t_star_and_theta_t1_star: float, y_t: float) -> float:
+    """The closing arithmetic of ``EMMREvaluator.evaluate`` (emmr.py:198-237): ``mean_t`` and ``var_t`` are the
+    posterior of the GP over all t trials at theta*_t, theta*_{t-1} and x_t, ``kappa_t1`` and
+    ``mu_t1_theta_t1_star`` come from the GP over the first t - 1 trials."""
+    mu_t_theta_t_star, variance_t_theta_t_star = float(mean_t[0]), float(var_t[0])
+    variance_t_theta_t1_star = float(var_t[1])
+    mu_t1_theta_t_with_nu_t, variance_t1_theta_t_with_nu_t = float(mean_t[2]), float(var_t[2])
+
+    theorem1_delta_mu_t_star = mu_t1_theta_t1_star - mu_t_theta_t_star
+    alg1_delta_r_tilde_t_term1 = theorem1_delta_mu_t_star
+    theorem1_v = math.sqrt(
+        max(
+            1e-10,
+            variance_t_theta_t_star
+            - 2.0 * cov_t_between_theta_t_star_and_theta_t1_star
+            + variance_t_theta_t1_star,
         )
-        theorem1_g = (mu_t_theta_t_star - mu_t1_theta_t1_star) / theorem1_v
-        alg1_delta_r_tilde_t_term2 = theorem1_v * scipy.stats.norm.pdf(theorem1_g)
-        alg1_delta_r_tilde_t_term3 = theorem1_v * theorem1_g * scipy.stats.norm.cdf(theorem1_g)
+    )
+    theorem1_g = (mu_t_theta_t_star - mu_t1_theta_t1_star) / theorem1_v
+    alg1_delta_r_tilde_t_term2 = theorem1_v * scipy.stats.norm.pdf(theorem1_g)
+    alg1_delta_r_tilde_t_term3 = theorem1_v * theorem1_g * scipy.stats.norm.cdf(theorem1_g)
 
-        _lambda = prior.DEFAULT_MINIMUM_NOISE_VAR**-1
-        eq4_rhs_term1 = 0.5 * math.log(1.0 + _lambda * variance_t1_theta_t_with_nu_t)
-        eq4_rhs_term2 = -0.5 * variance_t1_theta_t_with_nu_t / (variance_t1_theta_t_with_nu_t + _lambda**-1)
-        eq4_rhs_term3 = (
-            0.5
-            * variance_t1_theta_t_with_nu_t
-            * (y_t - mu_t1_theta_t_with_nu_t) ** 2
-            / (variance_t1_theta_t_with_nu_t + _lambda**-1) ** 2
-        )
-        alg1_delta_r_tilde_t_term4 = kappa_t1 * math.sqrt(0.5 * (eq4_rhs_term1 + eq4_rhs_term2 + eq4_rhs_term3))
+    _lambda = prior.DEFAULT_MINIMUM_NOISE_VAR**-1
+    eq4_rhs_term1 = 0.5 * math.log(1.0 + _lambda * variance_t1_theta_t_with_nu_t)
+    eq4_rhs_term2 = -0.5 * variance_t1_theta_t_with_nu_t / (variance_t1_theta_t_with_nu_t + _lambda**-1)
+    eq4_rhs_term3 = (
+        0.5
+        * variance_t1_theta_t_with_nu_t
+        * (y_t - mu_t1_theta_t_with_nu_t) ** 2
+        / (variance_t1_theta_t_with_nu_t + _lambda**-1) ** 2
+    )
+    alg1_delta_r_tilde_t_term4 = kappa_t1 * math.sqrt(0.5 * (eq4_rhs_term1 + eq4_rhs_term2 + eq4_rhs_term3))
 
-        return min(
-            sys.float_info.max * 0.5,
-            alg1_delta_r_tilde_t_term1
-            + alg1_delta_r_tilde_t_term2
-            + alg1_delta_r_tilde_t_term3
-            + alg1_delta_r_tilde_t_term4,
-        )
-
+    return min(
+        sys.float_info.max * 0.5,
+        alg1_delta_r_tilde_t_term1
+        + alg1_delta_r_tilde_t_term2
+        + alg1_delta_r_tilde_t_term3
+        + alg1_delta_r_tilde_t_term4,
+    )
 
 
 # ---- the whole improvement curve at once ------------------------------------------------------------------------------
@@ -341,76 +347,150 @@ class _Prefix:
 
 
 class _LockStep:
-    """Lock-step L-BFGS-B: one scipy fit per GP in its own thread.  A thread's loss call posts its raw parameters and
-    blocks; ``run`` evaluates everything posted in one ``gp_batch_loss``, then releases the threads one at a time and
-    waits for each to post again or finish.  So one fit thread runs at a time (the host work is serial under the GIL
-    anyway) and the threads do not contend for the GIL; a thread whose fit has returned leaves the batch."""
+    """Lock-step L-BFGS-B: one scipy fit thread per task.  A thread's loss call posts the GP it fits and its raw
+    parameters and blocks; ``run`` evaluates everything posted in one ``gp_batch_loss``, then releases the threads one
+    at a time and waits for each to post again or finish.  So one fit thread runs at a time (the host work is serial
+    under the GIL anyway) and the threads do not contend for the GIL; a thread whose task has returned leaves the
+    batch.  With ``deterministic`` every fit holds the noise at ``minimum_noise`` (the fixed-noise batched loss)."""
 
-    def __init__(self, engine, minimum_noise: float) -> None:
+    def __init__(self, engine, minimum_noise: float, deterministic: bool = False) -> None:
         self._engine = engine
         self._minimum_noise = minimum_noise
+        self.deterministic = deterministic
         self._cond = threading.Condition()
-        self._posted: dict[int, np.ndarray] = {}
+        self._posted: dict[int, tuple[int, np.ndarray]] = {}
         self._left: set[int] = set()
         self._results: dict[int, tuple] = {}
         self._events: dict[int, threading.Event] = {}
         self.rounds = 0
         self.device_seconds = 0.0
 
-    def slot(self, gp: int) -> "_Slot":
-        self._events[gp] = threading.Event()
-        return _Slot(self, gp)
+    def slot(self, key: int) -> "_Slot":
+        self._events[key] = threading.Event()
+        return _Slot(self, key)
 
-    def post(self, gp: int, raw: np.ndarray):
-        ev = self._events[gp]
+    def post(self, key: int, gp: int, raw: np.ndarray):
+        ev = self._events[key]
         with self._cond:
-            self._posted[gp] = raw
+            self._posted[key] = (gp, raw)
             self._cond.notify()
         ev.wait()
         ev.clear()
-        return self._results.pop(gp)
+        return self._results.pop(key)
 
-    def leave(self, gp: int) -> None:
+    def leave(self, key: int) -> None:
         with self._cond:
-            self._left.add(gp)
+            self._left.add(key)
             self._cond.notify()
 
-    def _wait(self, gp: int) -> None:
+    def _wait(self, key: int) -> None:
         with self._cond:
-            while gp not in self._posted and gp not in self._left:
+            while key not in self._posted and key not in self._left:
                 self._cond.wait()
 
     def run(self, threads: list) -> None:
         import time
-        for gp, th in enumerate(threads):
+        for key, th in enumerate(threads):
             th.start()
-            self._wait(gp)
+            self._wait(key)
         while self._posted:
             batch, self._posted = self._posted, {}
-            gps = sorted(batch)
+            keys = sorted(batch)
+            gps = [batch[k][0] for k in keys]
+            raws = np.stack([batch[k][1] for k in keys])
             t0 = time.perf_counter()
-            loss, grad, status = self._engine.gp_batch_loss(gps, np.stack([batch[g] for g in gps]),
-                                                            self._minimum_noise)
+            if self.deterministic:
+                loss, grad, status = self._engine.gp_batch_loss(gps, raws, self._minimum_noise, deterministic=True)
+            else:
+                loss, grad, status = self._engine.gp_batch_loss(gps, raws, self._minimum_noise)
             self.device_seconds += time.perf_counter() - t0
             self.rounds += 1
-            for i, g in enumerate(gps):
-                self._results[g] = (float(loss[i]), grad[i].copy(), int(status[i]))
-                self._events[g].set()
-                self._wait(g)
+            for i, k in enumerate(keys):
+                self._results[k] = (float(loss[i]), grad[i].copy(), int(status[i]))
+                self._events[k].set()
+                self._wait(k)
 
 
 class _Slot:
-    """The engine a fit thread sees: ``gp_loss`` answered by the lock-step batch."""
+    """The engine a fit thread sees: ``gp_loss`` answered by the lock-step batch, for the GP ``gp`` of the wave
+    (the thread's own index unless its task sets another)."""
 
-    def __init__(self, lockstep: _LockStep, gp: int) -> None:
+    def __init__(self, lockstep: _LockStep, key: int) -> None:
         self._ls = lockstep
-        self._gp = gp
+        self._key = key
+        self.gp = key
 
-    def gp_loss(self, raw_params, minimum_noise: float):
-        loss, grad, status = self._ls.post(self._gp, np.array(raw_params, dtype=np.float64))
+    def gp_loss(self, raw_params, minimum_noise: float, deterministic: bool = False):
+        if deterministic != self._ls.deterministic:
+            raise ValueError("a fit's noise model differs from its lock-step batch's")
+        loss, grad, status = self._ls.post(self._key, self.gp, np.array(raw_params, dtype=np.float64))
         if status:
             raise GPCholeskyError("the GP covariance is not positive definite")
         return loss, grad
+
+
+def _in_waves(device: int, units: list[tuple[int, int]], run_wave, stats: dict | None) -> None:
+    """The driver both batched evaluators use.  ``units`` holds (P, device bytes) per unit of work (a distinct
+    complete set); the units are grouped by P in first-seen order and packed into waves of at most ``_WAVE_BYTES``
+    (a unit larger than that gets a wave of its own), and ``run_wave(engine, wave)`` runs each wave's unit indices on
+    one engine, under one BLAS thread limit."""
+    import time
+    by_p: dict[int, list[int]] = {}
+    for i, (P, _) in enumerate(units):
+        by_p.setdefault(P, []).append(i)
+    engine = _engine_cls(device)
+    t_all = time.perf_counter()
+    try:
+        with single_blas_thread_if_scipy_v1_15_or_newer():
+            for members in by_p.values():
+                waves: list[list[int]] = [[]]
+                used = 0
+                for i in members:
+                    need = units[i][1]
+                    if waves[-1] and used + need > _WAVE_BYTES:
+                        waves.append([])
+                        used = 0
+                    waves[-1].append(i)
+                    used += need
+                for wave in waves:
+                    run_wave(engine, wave)
+    finally:
+        engine.close()
+    if stats is not None:
+        stats["wall_seconds"] = time.perf_counter() - t_all
+
+
+def _fit_wave(engine, data: list[tuple[np.ndarray, np.ndarray]], is_categorical, minimum_noise: float, tasks: list,
+              stats: dict | None, deterministic: bool = False) -> list:
+    """Uploads a wave's GPs (GP i fitted to ``data[i]`` = (X, y)) and runs ``tasks[k](slot)`` for every k, each in its
+    own thread, in lock step.  A task fits through its slot, choosing the GP by ``slot.gp``.  Returns the tasks'
+    results in order; an exception of a task is re-raised, the first task's first."""
+    offsets = np.zeros(len(data) + 1, dtype=np.int64)
+    offsets[1:] = np.cumsum([X.shape[0] for X, _ in data])
+    engine.gp_batch_set(offsets, np.concatenate([X for X, _ in data]), np.concatenate([y for _, y in data]),
+                        is_categorical)
+    ls = _LockStep(engine, minimum_noise, deterministic)
+    results: dict[int, object] = {}
+    errors: dict[int, BaseException] = {}
+
+    def work(k: int, slot: _Slot) -> None:
+        try:
+            results[k] = tasks[k](slot)
+        except BaseException as e:   # re-raised below, in task order
+            errors[k] = e
+        finally:
+            ls.leave(k)
+
+    threads = [threading.Thread(target=work, args=(k, ls.slot(k)), daemon=True) for k in range(len(tasks))]
+    ls.run(threads)
+    for th in threads:
+        th.join()
+    if errors:
+        raise errors[min(errors)]
+    if stats is not None:
+        stats["rounds"] = stats.get("rounds", 0) + ls.rounds
+        stats["device_seconds"] = stats.get("device_seconds", 0.0) + ls.device_seconds
+    return [results[k] for k in range(len(tasks))]
 
 
 def _prepare_prefixes(evaluator: "RegretBoundEvaluator", study) -> tuple[list[int], list[_Prefix]]:
@@ -455,7 +535,6 @@ def _prepare_prefixes(evaluator: "RegretBoundEvaluator", study) -> tuple[list[in
 
 
 def _batched_improvements(evaluator: "RegretBoundEvaluator", study, stats: dict | None = None) -> tuple[list, list]:
-    import time
     rng = evaluator._rng.rng
     start_state = rng.get_state()
     trial_numbers, prefixes = _prepare_prefixes(evaluator, study)
@@ -467,35 +546,16 @@ def _batched_improvements(evaluator: "RegretBoundEvaluator", study, stats: dict 
         if not gps or p.X is not gps[-1].X:
             gps.append(p)
         p.gp = len(gps) - 1
-    by_p: dict[int, list[int]] = {}
-    for i, g in enumerate(gps):
-        by_p.setdefault(g.X.shape[1], []).append(i)
     params: list[np.ndarray | None] = [None] * len(gps)
     n_samples = evaluator._optimize_n_samples
     out = np.empty((len(prefixes), 3))
     users = [[] for _ in gps]
     for j, p in enumerate(prefixes):
         users[p.gp].append(j)
-    engine = _engine_cls(evaluator._device)
-    t_all = time.perf_counter()
-    try:
-        with single_blas_thread_if_scipy_v1_15_or_newer():
-            for P, members in by_p.items():
-                waves: list[list[int]] = [[]]
-                used = 0
-                for i in members:
-                    need = _wave_bytes(gps[i].X.shape[0], P, n_samples * len(users[i]))
-                    if waves[-1] and used + need > _WAVE_BYTES:
-                        waves.append([])
-                        used = 0
-                    waves[-1].append(i)
-                    used += need
-                for wave in waves:
-                    _run_wave(engine, evaluator, gps, wave, users, prefixes, params, out, stats)
-    finally:
-        engine.close()
-    if stats is not None:
-        stats["wall_seconds"] = time.perf_counter() - t_all
+    units = [(g.X.shape[1], _wave_bytes(g.X.shape[0], g.X.shape[1], n_samples * len(users[i])))
+             for i, g in enumerate(gps)]
+    _in_waves(evaluator._device, units,
+              lambda engine, wave: _run_wave(engine, evaluator, gps, wave, users, prefixes, params, out, stats), stats)
     # the reference raises at the first prefix whose final covariance is not positive definite, after drawing that
     # prefix's samples: leave the stream there
     for j, p in enumerate(prefixes):
@@ -536,40 +596,197 @@ def _prepare_prefixes_upto(evaluator, study, last: int) -> None:
 def _run_wave(engine, evaluator, gps, wave, users, prefixes, params, out, stats) -> None:
     """Fits the GPs of one wave in lock step, then the bounds of every prefix that uses them."""
     P = gps[wave[0]].X.shape[1]
-    offsets = np.zeros(len(wave) + 1, dtype=np.int64)
-    offsets[1:] = np.cumsum([gps[i].X.shape[0] for i in wave])
-    engine.gp_batch_set(offsets, np.concatenate([gps[i].X for i in wave]), np.concatenate([gps[i].y for i in wave]),
-                        gps[wave[0]].is_categorical)
-    ls = _LockStep(engine, evaluator._minimum_noise)
-    results: dict[int, np.ndarray] = {}
-    errors: dict[int, BaseException] = {}
 
-    def work(local: int, slot: _Slot) -> None:
-        try:
-            results[local] = _fit(slot, P, evaluator._log_prior, evaluator._minimum_noise, single_blas=False)
-        except BaseException as e:   # re-raised below, in prefix order
-            errors[local] = e
-        finally:
-            ls.leave(local)
+    def task(slot: _Slot) -> np.ndarray:
+        return _fit(slot, P, evaluator._log_prior, evaluator._minimum_noise, single_blas=False)
 
-    threads = [threading.Thread(target=work, args=(k, ls.slot(k)), daemon=True) for k in range(len(wave))]
-    ls.run(threads)
-    for th in threads:
-        th.join()
-    if errors:
-        raise errors[min(errors)]
-    if stats is not None:
-        stats["rounds"] = stats.get("rounds", 0) + ls.rounds
-        stats["device_seconds"] = stats.get("device_seconds", 0.0) + ls.device_seconds
+    fitted = _fit_wave(engine, [(gps[i].X, gps[i].y) for i in wave], gps[wave[0]].is_categorical,
+                       evaluator._minimum_noise, [task] * len(wave), stats)
     jobs = [(k, j) for k, i in enumerate(wave) for j in users[i]]
     idx = np.array([k for k, _ in jobs], dtype=np.int32)
-    prm = np.stack([results[k] for k, _ in jobs])
+    prm = np.stack([fitted[k] for k, _ in jobs])
     beta = np.array([prefixes[j].beta for _, j in jobs])
     samples = np.stack([prefixes[j].samples for _, j in jobs])
     res, status = engine.gp_batch_bounds(idx, prm, beta, samples)
     for r, (k, j), st in zip(res, jobs, status):
         out[j] = r
         prefixes[j].failed = bool(st)
+
+
+# ---- EMMR: both Gaussian processes of every prefix ----------------------------------------------------------------
+
+_EMMR_N_SAMPLES = 2048   # the samples of _compute_standardized_regret_bound that EMMREvaluator.evaluate draws
+
+
+def _emmr_wave_bytes(t: int, P: int, n_users: int) -> int:
+    """Device bytes one complete set of t trials adds to a wave: the rows of both its GPs (t - 1 and t), their loss
+    workspace (tpe_gpbatch.cuh: an n x n matrix and three n-vectors above 160 rows), per prefix that uses the set the
+    bounds workspace of the first GP (that again, n x 256 doubles of cross covariance) and its samples, and the two
+    moments jobs (the loss workspace and three n-vectors of cross covariance, tpe_gpemmr.cuh)."""
+    def ws(n: int) -> int:
+        return n * n + 3 * n if n > 160 else 0
+    rows = (2 * t - 1) * (P + 1)
+    loss = ws(t - 1) + ws(t)
+    bounds = n_users * (ws(t - 1) + 256 * (t - 1) + _EMMR_N_SAMPLES * P + 4)
+    moments = ws(t - 1) + ws(t) + 3 * (2 * t - 1) + 2 * (P + 2) + 24
+    return 8 * (rows + loss + bounds + moments + 4 * (P + 2) + 16)
+
+
+class _EMMRSet:
+    """What ``EMMREvaluator.evaluate`` forms from one complete set before its fits (emmr.py:141-186): the data of
+    both GPs, the two argmax rows and beta; after the fits, what it reads from them."""
+
+    __slots__ = ("X", "y", "is_categorical", "theta_t_star", "theta_t1_star", "beta", "users", "failed",
+                 "mu_t1_theta_t1_star", "mean_t", "var_t", "cov_t")
+
+
+class _EMMRPrefix:
+    """One trial prefix of the EMMR curve: a constant (too few complete trials, or no search space), or a set, its
+    own samples, and the stream state just after drawing them."""
+
+    __slots__ = ("value", "set", "samples", "state", "kappa", "failed")
+
+
+def _prepare_emmr(evaluator: "EMMREvaluator", study, error_evaluator=None):
+    """The host pre-pass, in trial order: per prefix what ``EMMREvaluator.evaluate`` does before its fits, with the
+    same warnings and the same draws from the evaluator's stream.  With ``error_evaluator`` it is called after each
+    prefix, as the reference loop calls it, so that an error evaluator sharing the stream (``MedianErrorEvaluator``
+    of this evaluator) draws where it draws there."""
+    trial_numbers: list[int] = []
+    prefixes: list[_EMMRPrefix] = []
+    errors: list[float] = []
+    completed: list[FrozenTrial] = []
+    rng = evaluator._rng.rng
+    direction = study.direction
+    last_n = -1
+    space = score_vals_raw = cur = None
+    for trial in study.trials:
+        if trial.state == TrialState.COMPLETE:
+            completed.append(trial)
+        if not completed:
+            continue
+        trial_numbers.append(trial.number)
+        p = _EMMRPrefix()
+        p.value, p.set, p.failed = None, None, False
+        t = len(completed)
+        if t < evaluator.min_n_trials:
+            p.value = sys.float_info.max * MARGIN_FOR_NUMARICAL_STABILITY  # Do not terminate.
+        else:
+            if t != last_n:
+                space = gp_search_space.SearchSpace(intersection_search_space(completed))
+                sign = -1 if direction == StudyDirection.MINIMIZE else 1
+                score_vals_raw = np.array([tr.value for tr in completed]) * sign
+                cur = None
+                last_n = t
+            if not space.dim:
+                optuna_warn(
+                    f"{evaluator.__class__.__name__} cannot consider any search space."
+                    "Termination will never occur in this study."
+                )
+                p.value = sys.float_info.max * MARGIN_FOR_NUMARICAL_STABILITY  # Do not terminate.
+            else:
+                # the reference converts (and warns) at every evaluate, shared set or not
+                score_vals = gp.warn_and_convert_inf(score_vals_raw)
+                if cur is None:
+                    cur = _EMMRSet()
+                    cur.X = space.get_normalized_params(completed)
+                    cur.y = (score_vals - score_vals.mean()) / max(sys.float_info.min, score_vals.std())
+                    cur.is_categorical = space.is_categorical
+                    cur.theta_t_star = int(np.argmax(cur.y))
+                    cur.theta_t1_star = int(np.argmax(cur.y[:-1]))
+                    cur.beta = _get_beta(cur.X.shape[1], t - 1, evaluator._delta)
+                    cur.users = []
+                    cur.failed = False
+                p.set = cur
+                cur.users.append(len(prefixes))
+                p.samples = space.sample_normalized_params(_EMMR_N_SAMPLES, rng=rng)
+                p.state = rng.get_state()
+        prefixes.append(p)
+        if error_evaluator is not None:
+            errors.append(error_evaluator.evaluate(trials=completed, study_direction=direction))
+    return trial_numbers, prefixes, errors
+
+
+def _run_emmr_wave(engine, evaluator, sets: list[_EMMRSet], wave: list[int], prefixes, stats) -> None:
+    """Fits both GPs of every set of one wave in lock step (GP 2k over the first t - 1 trials of set k, GP 2k + 1 over
+    all t, warm-started from the first), then every prefix's kappa in one bounds launch and every set's posterior
+    terms in one moments launch."""
+    P = sets[wave[0]].X.shape[1]
+    minimum_noise = prior.DEFAULT_MINIMUM_NOISE_VAR
+    det = evaluator._deterministic
+
+    def task(k: int):
+        def fit_both(slot: _Slot):
+            slot.gp = 2 * k
+            params_t1 = _fit(slot, P, prior.default_log_prior, minimum_noise, deterministic_objective=det,
+                             single_blas=False)
+            slot.gp = 2 * k + 1
+            params_t = _fit(slot, P, prior.default_log_prior, minimum_noise, gpr_cache=params_t1,
+                            deterministic_objective=det, single_blas=False)
+            return params_t1, params_t
+        return fit_both
+
+    data = []
+    for i in wave:
+        s = sets[i]
+        data += [(s.X[:-1], s.y[:-1]), (s.X, s.y)]
+    fitted = _fit_wave(engine, data, sets[wave[0]].is_categorical, minimum_noise,
+                       [task(k) for k in range(len(wave))], stats, deterministic=det)
+
+    # kappa of every prefix: the regret bound of the first GP over its train rows and the prefix's samples
+    jobs = [(k, j) for k, i in enumerate(wave) for j in sets[i].users]
+    res, status = engine.gp_batch_bounds(np.array([2 * k for k, _ in jobs], dtype=np.int32),
+                                         np.stack([fitted[k][0] for k, _ in jobs]),
+                                         np.array([sets[wave[k]].beta for k, _ in jobs]),
+                                         np.stack([prefixes[j].samples for _, j in jobs]))
+    for r, (_, j), st in zip(res, jobs, status):
+        prefixes[j].kappa = max(r[0], r[1]) - r[2]
+        prefixes[j].failed = bool(st)
+    # the first GP at theta*_{t-1}; the second at theta*_t, theta*_{t-1} and x_t, with the joint covariance of the
+    # first two
+    idx, prm, rows = [], [], []
+    for k, i in enumerate(wave):
+        s = sets[i]
+        idx += [2 * k, 2 * k + 1]
+        prm += [fitted[k][0], fitted[k][1]]
+        rows += [[s.theta_t1_star] * 3, [s.theta_t_star, s.theta_t1_star, s.X.shape[0] - 1]]
+    mean, var, cov, status = engine.gp_batch_moments(np.array(idx, dtype=np.int32), np.stack(prm),
+                                                     np.array(rows, dtype=np.int32), 2)
+    for k, i in enumerate(wave):
+        s = sets[i]
+        s.failed = bool(status[2 * k] or status[2 * k + 1])
+        s.mu_t1_theta_t1_star = float(mean[2 * k, 0])
+        s.mean_t, s.var_t, s.cov_t = mean[2 * k + 1], var[2 * k + 1], cov[2 * k + 1]
+
+
+def _batched_emmr(evaluator: "EMMREvaluator", study, error_evaluator=None,
+                  stats: dict | None = None) -> tuple[list, list, list]:
+    """``_get_improvement_info``'s walk with ``EMMREvaluator.evaluate`` at every prefix: the pre-pass, both fits of
+    every distinct complete set in lock step, then the closing arithmetic per prefix."""
+    trial_numbers, prefixes, errors = _prepare_emmr(evaluator, study, error_evaluator)
+    sets: list[_EMMRSet] = []
+    for p in prefixes:
+        if p.set is not None and (not sets or p.set is not sets[-1]):
+            sets.append(p.set)
+    if sets:
+        units = [(s.X.shape[1], _emmr_wave_bytes(s.X.shape[0], s.X.shape[1], len(s.users))) for s in sets]
+        _in_waves(evaluator._device, units,
+                  lambda engine, wave: _run_emmr_wave(engine, evaluator, sets, wave, prefixes, stats), stats)
+    improvements = []
+    for p in prefixes:
+        if p.set is None:
+            improvements.append(p.value)
+            continue
+        if p.failed or p.set.failed:
+            # the per-prefix evaluator raises after drawing this prefix's samples (between its two fits)
+            evaluator._rng.rng.set_state(p.state)
+            raise np.linalg.LinAlgError("Matrix is not positive definite")
+        s = p.set
+        # emmr.py:249-250: for one point the reference takes the variance of the non-joint posterior
+        cov_t_between = float(s.var_t[0] if s.theta_t_star == s.theta_t1_star else s.cov_t[0, 1])
+        improvements.append(_emmr_criterion(p.kappa, s.mu_t1_theta_t1_star, s.mean_t, s.var_t, cov_t_between,
+                                            s.y[-1]))
+    return trial_numbers, improvements, errors
 
 
 def terminator_improvement_history(study, improvement_evaluator=None, error_evaluator=None, get_error: bool = False):
@@ -580,9 +797,20 @@ def terminator_improvement_history(study, improvement_evaluator=None, error_eval
     With the default evaluator, or an evaluator whose type is exactly ``optuna_b200.RegretBoundEvaluator``, the
     Gaussian processes of every trial prefix are fitted together: the host forms each prefix's data and draws its
     samples from the evaluator's stream in the reference's order, then one device launch per L-BFGS-B round
-    evaluates every live fit (``tpe_gp_batch_loss``) and one more gives every prefix's bounds.  Any other improvement
-    evaluator takes optuna's per-prefix loop unchanged.  Error evaluators are called per prefix, as the reference
-    calls them."""
+    evaluates every live fit (``tpe_gp_batch_loss``) and one more gives every prefix's bounds.  Error evaluators are
+    then called per prefix.
+
+    With an evaluator whose type is exactly ``optuna_b200.EMMREvaluator``, both Gaussian processes of every prefix
+    (over all complete trials but the last, then over all of them, warm-started from the first) are fitted in lock
+    step: the host forms each prefix's data, emits the reference's warnings and draws its samples in trial order, one
+    launch per L-BFGS-B round evaluates every live fit of either kind (``tpe_gp_batch_loss``, or
+    ``tpe_gp_batch_loss_fixed_noise`` with ``deterministic_objective``), then one bounds launch gives every prefix's
+    regret bound and one moments launch (``tpe_gp_batch_moments``) every posterior term the criterion reads.  The
+    error evaluator is called after each prefix's draws, as the reference loop calls it, so that a
+    ``MedianErrorEvaluator`` paired with the same evaluator draws from the shared stream where it draws there.
+
+    Any other improvement evaluator (optuna's own, or a subclass of these) takes optuna's per-prefix loop
+    unchanged."""
     from optuna.terminator import CrossValidationErrorEvaluator, StaticErrorEvaluator
     from optuna.terminator.improvement.evaluator import BestValueStagnationEvaluator
     from optuna.visualization._terminator_improvement import _get_improvement_info, _ImprovementInfo
@@ -596,6 +824,10 @@ def terminator_improvement_history(study, improvement_evaluator=None, error_eval
             error_evaluator = StaticErrorEvaluator(constant=0)
         else:
             error_evaluator = CrossValidationErrorEvaluator()
+    if type(improvement_evaluator) is EMMREvaluator:
+        trial_numbers, improvements, errors = _batched_emmr(improvement_evaluator, study,
+                                                            error_evaluator if get_error else None)
+        return _ImprovementInfo(trial_numbers=trial_numbers, improvements=improvements, errors=errors or None)
     if type(improvement_evaluator) is not RegretBoundEvaluator:
         return _get_improvement_info(study, get_error, improvement_evaluator, error_evaluator)
     trial_numbers, improvements = _batched_improvements(improvement_evaluator, study)
