@@ -45,7 +45,8 @@ extern "C" {
 /* 14: + tpe_box_decomposition, tpe_get_box_decomposition */
 /* 15: + tpe_gp_batch_set, tpe_gp_batch_loss, tpe_gp_batch_bounds */
 /* 16: + tpe_gp_batch_loss_fixed_noise, tpe_gp_batch_moments */
-#define TPE_ABI_VERSION 16
+/* 17: + tpe_acqf_set, tpe_acqf_eval */
+#define TPE_ABI_VERSION 17
 
 enum {
   TPE_OK = 0,
@@ -390,6 +391,26 @@ int tpe_gp_batch_moments(tpe_ctx* ctx, int64_t k, const int32_t* gp_idx, const d
 int tpe_ehvi_set(tpe_ctx* ctx, const double* lower, const double* intervals, int64_t B, const double* samples,
                  int32_t S, int32_t M);
 int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, double* value, double* dmean, double* dsd);
+/* GPSampler's acquisition function (optuna/_gp/acqf.py) over the posteriors of conditioned GP contexts, fp64, with its
+ * gradient in the query point.  Kept apart from every other state of the acquisition context except its log-EHVI
+ * boxes and samples, which tpe_acqf_set replaces for TPE_ACQF_LOGEHVI.
+ * tpe_acqf_set: kind TPE_ACQF_LOGEI (n_obj = 1: LogEI of gps[0], acqf.py:151-159), TPE_ACQF_LOGEHVI (2 <= n_obj <= 24:
+ * log-EHVI of gps[0 .. n_obj - 1] over lower / intervals [B, M] and samples [S, M] as tpe_ehvi_set takes them) or
+ * TPE_ACQF_LOGPI (n_obj = 0: no objective part).  gps[n_obj .. n_gp - 1] are constraints: their LogPI terms
+ * (acqf.py:175-182) are summed as ConstrainedLogEI / ConstrainedLogEHVI sum them.  thresholds [n_gp]: LogEI's f0
+ * (-inf gives the reference's zeros), then the constraints' thresholds (finite).  stabilizing_noise is added to every
+ * variance.  Every GP context must be conditioned (tpe_gp_condition), distinct, of one width P and on this context's
+ * device, and must outlive the calls; TPE_E_STATE / TPE_E_INVALID naming the violated condition.
+ * tpe_acqf_eval: value [Q] at the rows of X [Q, P] and, with grad non-NULL, d value / dx [Q, P].  The GP posteriors
+ * are computed on this context's stream after the work queued on each GP context's stream, with one synchronise per
+ * call.  A row's value is the same bits whatever Q, the row's position and the gradient request.  TPE_E_STATE when a
+ * GP context was conditioned again or changed since tpe_acqf_set; TPE_E_INVALID for Q < 1, or naming the bytes when
+ * the device lacks the memory.  Non-finite entries of X are evaluated: NaN propagates as in torch. */
+enum { TPE_ACQF_LOGEI = 0, TPE_ACQF_LOGEHVI = 1, TPE_ACQF_LOGPI = 2 };
+int tpe_acqf_set(tpe_ctx* ctx, int32_t kind, tpe_ctx* const* gps, int32_t n_gp, int32_t n_obj,
+                 const double* thresholds, double stabilizing_noise, const double* lower, const double* intervals,
+                 int64_t B, const double* samples, int32_t S);
+int tpe_acqf_eval(tpe_ctx* ctx, const double* X, int64_t Q, double* value, double* grad);
 /* Non-dominated box decomposition of LogEHVI (get_non_dominated_box_bounds, optuna/_hypervolume/box_decomposition.py:
  * 138-157, as optuna/_gp/acqf.py:255-263 calls it).  Kept apart from every other state of the context.
  * tpe_box_decomposition decomposes the space that the rows of loss_vals [n, M] (minimised) do not dominate, below

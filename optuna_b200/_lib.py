@@ -83,6 +83,9 @@ SYMBOLS = {
     "tpe_gp_query": (C.c_int, [_P, _P, C.c_int64, _P, _P, _P, _P]),
     "tpe_ehvi_set": (C.c_int, [_P, _P, _P, C.c_int64, _P, C.c_int32, C.c_int32]),
     "tpe_ehvi": (C.c_int, [_P, _P, _P, C.c_int64, _P, _P, _P]),
+    "tpe_acqf_set": (C.c_int, [_P, C.c_int32, _P, C.c_int32, C.c_int32, _P, C.c_double, _P, _P, C.c_int64, _P,
+                               C.c_int32]),
+    "tpe_acqf_eval": (C.c_int, [_P, _P, C.c_int64, _P, _P]),
     "tpe_box_decomposition": (C.c_int, [_P, _P, C.c_int64, C.c_int32, _P, C.POINTER(C.c_int64)]),
     "tpe_get_box_decomposition": (C.c_int, [_P, _P, _P, _P]),
     "tpe_gp_batch_set": (C.c_int, [_P, C.c_int32, _P, C.c_int32, _P, _P, _P]),
@@ -100,7 +103,7 @@ SYMBOLS = {
 _lib = None
 
 
-ABI_VERSION = 16  # include/optuna_b200_tpe.h TPE_ABI_VERSION
+ABI_VERSION = 17  # include/optuna_b200_tpe.h TPE_ABI_VERSION
 
 
 def load() -> C.CDLL:

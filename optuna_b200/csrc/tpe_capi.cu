@@ -26,6 +26,7 @@
 #include "tpe_gpbatch.cuh"
 #include "tpe_gpemmr.cuh"
 #include "tpe_ehvi.cuh"
+#include "tpe_acqf.cuh"
 #include "tpe_boxdec.cuh"
 #include "tpe_uni.cuh"
 #include "tpe_mixed.cuh"
@@ -164,6 +165,24 @@ struct EhviState {
   void release() {
     for (DevBuf* b : {&lbI, &Z, &mean, &sd, &part, &value, &dmean, &dsd}) b->release();
     *this = EhviState();
+  }
+};
+
+// GPSampler's acquisition function (tpe_acqf_*, tpe_acqf.cuh): the GP contexts of tpe_acqf_set with the conditioning
+// generation each had then, one event per GP context, the thresholds, and the per-call buffers of tpe_acqf_eval.  The
+// log-EHVI boxes and samples live in the context's EhviState.
+struct AcqfState {
+  int32_t kind = 0, n_obj = 0, P = 0;
+  double noise = 0.0;
+  std::vector<tpe_ctx*> gps;
+  std::vector<uint64_t> gen;
+  std::vector<cudaEvent_t> ev;
+  DevBuf thr, X, mean, var, dmean, dvar, coef, value, grad;
+  bool ready = false;
+  void release() {
+    for (DevBuf* b : {&thr, &X, &mean, &var, &dmean, &dvar, &coef, &value, &grad}) b->release();
+    for (cudaEvent_t e : ev) cudaEventDestroy(e);
+    *this = AcqfState();
   }
 };
 
@@ -318,9 +337,11 @@ struct tpe_ctx {
   int32_t uni_ord_col = -1;
   int64_t uni_ord_K = -1;
   GpState gp;
+  uint64_t gp_generation = 0;   // successful tpe_gp_condition calls: an acquisition context checks it is unchanged
   GpBatchState gpb;
   EhviState ehvi;
   BoxDecState boxdec;
+  AcqfState acqf;
 };
 
 namespace {
@@ -2470,6 +2491,7 @@ void tpe_ctx_destroy(tpe_ctx* ctx) {
   ctx->gp.release();
   ctx->gpb.release();
   ctx->ehvi.release();
+  ctx->acqf.release();
   ctx->boxdec.release();
   if (ctx->res_host) cudaFreeHost(ctx->res_host);
   if (ctx->mt_host) cudaFreeHost(ctx->mt_host);
@@ -4112,6 +4134,7 @@ int tpe_gp_condition(tpe_ctx* ctx, const double* params) {
   CU(cudaStreamSynchronize(st));
   if (failed) return fail(ctx, TPE_E_NOTPD, "the GP covariance is not positive definite (Cholesky pivot <= 0 or NaN)");
   g.conditioned = true;
+  ++ctx->gp_generation;
   return TPE_OK;
 }
 
@@ -4428,10 +4451,9 @@ static EhviChunkFn ehvi_chunk_kernel(int M, bool grad) {
 }
 
 // replaces LogEHVI.__init__'s state (optuna/_gp/acqf.py:245-280): the non-dominated boxes and the fixed QMC samples
-int tpe_ehvi_set(tpe_ctx* ctx, const double* lower, const double* intervals, int64_t B, const double* samples,
-                 int32_t S, int32_t M) {
-  if (!ctx) return TPE_E_INVALID;
-  std::lock_guard<std::mutex> lk(ctx->mu);
+// The body of tpe_ehvi_set, called under the context lock (also by tpe_acqf_set)
+static int ehvi_upload(tpe_ctx* ctx, const double* lower, const double* intervals, int64_t B, const double* samples,
+                       int32_t S, int32_t M) {
   EhviState& e = ctx->ehvi;
   e.ready = false;
   if (M < 2 || M > ehvi::MAX_M) return fail(ctx, TPE_E_INVALID, "EHVI needs 2 <= M <= %d objectives, got %d", ehvi::MAX_M, M);
@@ -4466,40 +4488,47 @@ int tpe_ehvi_set(tpe_ctx* ctx, const double* lower, const double* intervals, int
   return TPE_OK;
 }
 
-// replaces LogEHVI.eval_acqf after the posteriors (acqf.py:282-300, with logehvi :45-62) and its autograd backward in
-// the posterior mean and standard deviation
-int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, double* value, double* dmean,
-             double* dsd) {
+int tpe_ehvi_set(tpe_ctx* ctx, const double* lower, const double* intervals, int64_t B, const double* samples,
+                 int32_t S, int32_t M) {
   if (!ctx) return TPE_E_INVALID;
   std::lock_guard<std::mutex> lk(ctx->mu);
+  return ehvi_upload(ctx, lower, intervals, B, samples, S, M);
+}
+
+// The bytes ehvi_launch allocates for Q rows that the context does not hold yet
+static size_t ehvi_new_bytes(const EhviState& e, int64_t Q, bool grad, bool inputs) {
+  const int M = e.M, K = grad ? 1 + 2 * M : 1;
+  const int64_t nchunks = (e.B + ehvi::CHUNK - 1) / ehvi::CHUNK;
+  const int64_t slab = std::max<int64_t>(1, std::min<int64_t>({Q, kEhviPartDoubles / (nchunks * K), 65535}));
+  auto more = [](const DevBuf& b, size_t bytes) { return bytes > b.cap ? bytes : (size_t)0; };
+  size_t need = more(e.value, (size_t)Q * 8) + more(e.part, (size_t)slab * nchunks * K * 8);
+  if (inputs) need += more(e.mean, (size_t)Q * M * 8) + more(e.sd, (size_t)Q * M * 8);
+  if (grad) need += more(e.dmean, (size_t)Q * M * 8) + more(e.dsd, (size_t)Q * M * 8);
+  return need;
+}
+
+// log-EHVI at Q rows of device means and standard deviations [Q][M] into e.value and, with grad, e.dmean / e.dsd, on
+// the context stream
+static int ehvi_launch(tpe_ctx* ctx, const double* mean_d, const double* sd_d, int64_t Q, bool grad) {
   EhviState& e = ctx->ehvi;
-  if (!e.ready) return fail(ctx, TPE_E_STATE, "no EHVI boxes and samples (tpe_ehvi_set)");
-  if (!mean || !sd || !value || Q < 1 || (dmean == nullptr) != (dsd == nullptr))
-    return fail(ctx, TPE_E_INVALID, "bad EHVI arguments");
-  if (set_device(ctx)) return TPE_E_CUDA;
-  const bool grad = dmean != nullptr;
   const int M = e.M, K = grad ? 1 + 2 * M : 1;
   const int64_t nchunks = (e.B + ehvi::CHUNK - 1) / ehvi::CHUNK;
   // rows per launch: the partial sums stay under kEhviPartDoubles and the grid's y extent under 65 535
   const int64_t slab = std::max<int64_t>(1, std::min<int64_t>({Q, kEhviPartDoubles / (nchunks * K), 65535}));
   cudaStream_t st = ctx->stream;
-  CU(e.mean.ensure((size_t)Q * M * 8));
-  CU(e.sd.ensure((size_t)Q * M * 8));
   CU(e.value.ensure((size_t)Q * 8));
   CU(e.part.ensure((size_t)slab * nchunks * K * 8));
   if (grad) {
     CU(e.dmean.ensure((size_t)Q * M * 8));
     CU(e.dsd.ensure((size_t)Q * M * 8));
   }
-  CU(cudaMemcpyAsync(e.mean.p, mean, (size_t)Q * M * 8, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(e.sd.p, sd, (size_t)Q * M * 8, cudaMemcpyHostToDevice, st));
   const size_t smem = ehvi::smem_bytes(M, grad);
   const double log_s = std::log((double)e.S);
   for (int64_t r0 = 0; r0 < Q; r0 += slab) {
     const int64_t rows = std::min(slab, Q - r0);
     const dim3 grid((unsigned)nchunks, (unsigned)rows);
-    const double* m0 = e.mean.as<double>() + r0 * M;
-    const double* s0 = e.sd.as<double>() + r0 * M;
+    const double* m0 = mean_d + r0 * M;
+    const double* s0 = sd_d + r0 * M;
     const unsigned fb = (unsigned)((rows + 127) / 128);
     ehvi_chunk_kernel(M, grad)<<<grid, ehvi::THREADS, smem, st>>>(e.lbI.as<double>(), e.B, e.Z.as<double>(), e.S, M,
                                                                    m0, s0, e.part.as<double>());
@@ -4512,6 +4541,29 @@ int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, doub
                                                      e.value.as<double>() + r0, nullptr, nullptr);
     }
   }
+  return TPE_OK;
+}
+
+// replaces LogEHVI.eval_acqf after the posteriors (acqf.py:282-300, with logehvi :45-62) and its autograd backward in
+// the posterior mean and standard deviation
+int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, double* value, double* dmean,
+             double* dsd) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  EhviState& e = ctx->ehvi;
+  if (!e.ready) return fail(ctx, TPE_E_STATE, "no EHVI boxes and samples (tpe_ehvi_set)");
+  if (!mean || !sd || !value || Q < 1 || (dmean == nullptr) != (dsd == nullptr))
+    return fail(ctx, TPE_E_INVALID, "bad EHVI arguments");
+  if (set_device(ctx)) return TPE_E_CUDA;
+  const bool grad = dmean != nullptr;
+  const int M = e.M;
+  cudaStream_t st = ctx->stream;
+  CU(e.mean.ensure((size_t)Q * M * 8));
+  CU(e.sd.ensure((size_t)Q * M * 8));
+  CU(cudaMemcpyAsync(e.mean.p, mean, (size_t)Q * M * 8, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync(e.sd.p, sd, (size_t)Q * M * 8, cudaMemcpyHostToDevice, st));
+  const int rc = ehvi_launch(ctx, e.mean.as<double>(), e.sd.as<double>(), Q, grad);
+  if (rc != TPE_OK) return rc;
   CU(cudaGetLastError());
   CU(cudaMemcpyAsync(value, e.value.p, (size_t)Q * 8, cudaMemcpyDeviceToHost, st));
   if (grad) {
@@ -4520,6 +4572,187 @@ int tpe_ehvi(tpe_ctx* ctx, const double* mean, const double* sd, int64_t Q, doub
   }
   CU(cudaStreamSynchronize(st));
   return TPE_OK;
+}
+
+// ---- GPSampler's acquisition function over the device posteriors (tpe_acqf.cuh) --------------------------------------
+// The posterior of the conditioned GP g at the m rows Xq (device) on stream st, into mean / var [m] and, with dmean,
+// dmean / dvar [m][P]: gp_query_chunks' kernels in its chunks, on g's factor and scratch (A, W, part), with the
+// outputs in the caller's buffers.  A row's values are the same bits as tpe_gp_query's.
+static void acqf_posterior(cudaStream_t st, GpState& g, const double* Xq, int64_t m, double* mean, double* var,
+                           double* dmean, double* dvar) {
+  const int P = g.P;
+  const bool grad = dmean != nullptr;
+  const int64_t n = g.n, ntiles = (n + gp::NB - 1) / gp::NB, qmax = grad ? gp::NB : kGpQmax;
+  double* Wm = g.A + gp::NB * n;
+  for (int64_t q0 = 0; q0 < m; q0 += qmax) {
+    const int64_t Q = std::min(qmax, m - q0);
+    gp::k_gp_cross<<<dim3((unsigned)((n + 127) / 128), (unsigned)Q), 128, 0, st>>>(Xq + q0 * P, g.X, g.cat, g.prm, P,
+                                                                                  (int)n, (int)Q, g.A);
+    gp_gemm(st, g.A, n, g.B, n, g.part, 0, Q, n, n, 1.0, gp::GF_KHI_COL | gp::GF_SQSUM);
+    gp::k_gp_post_finish<<<(unsigned)((Q + 7) / 8), 256, 0, st>>>(g.A, g.alpha, g.part, (int)ntiles, g.prm, P, (int)n,
+                                                                  (int)Q, 0.0, true, mean + q0, var + q0);
+    if (grad) {
+      gp_gemm(st, g.A, n, g.B, n, g.W, n, Q, n, n, 1.0, gp::GF_KHI_COL);
+      gp_gemm(st, g.W, n, g.B, n, Wm, n, Q, n, n, 1.0, gp::GF_TB | gp::GF_KLO_COL);
+      const dim3 grid((unsigned)Q, (unsigned)((P + gp::GRAD_DC - 1) / gp::GRAD_DC));
+      gp::k_gp_post_grad<gp::GRAD_DC><<<grid, gp::GRAD_THREADS, 0, st>>>(
+          Xq + q0 * P, g.X, g.cat, g.prm, g.alpha, Wm, g.part, (int)ntiles, P, (int)n, dmean + q0 * P, dvar + q0 * P);
+    }
+  }
+}
+
+// replaces the state of GPSampler's acquisition functions (optuna/_gp/acqf.py: LogEI :116-149, ConstrainedLogEI
+// :217-235, LogEHVI :245-280, ConstrainedLogEHVI :303-331)
+int tpe_acqf_set(tpe_ctx* ctx, int32_t kind, tpe_ctx* const* gps, int32_t n_gp, int32_t n_obj,
+                 const double* thresholds, double stabilizing_noise, const double* lower, const double* intervals,
+                 int64_t B, const double* samples, int32_t S) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  AcqfState& a = ctx->acqf;
+  a.release();
+  if (kind < TPE_ACQF_LOGEI || kind > TPE_ACQF_LOGPI) return fail(ctx, TPE_E_INVALID, "unknown acquisition kind %d", kind);
+  const int want_obj = kind == TPE_ACQF_LOGEI ? 1 : kind == TPE_ACQF_LOGPI ? 0 : n_obj;
+  if (kind == TPE_ACQF_LOGEHVI && (n_obj < 2 || n_obj > ehvi::MAX_M))
+    return fail(ctx, TPE_E_INVALID, "log-EHVI needs 2 <= n_obj <= %d objectives, got %d", ehvi::MAX_M, n_obj);
+  if (n_obj != want_obj) return fail(ctx, TPE_E_INVALID, "acquisition kind %d takes %d objective GPs, got %d", kind,
+                                     want_obj, n_obj);
+  if (!gps || !thresholds || n_gp < std::max(n_obj, 1) || n_gp > 1 << 16)
+    return fail(ctx, TPE_E_INVALID, "bad acquisition arguments (%d GPs, %d objectives)", n_gp, n_obj);
+  if (!std::isfinite(stabilizing_noise) || stabilizing_noise < 0.0)
+    return fail(ctx, TPE_E_INVALID, "bad stabilizing noise");
+  for (int i = 0; i < n_gp; ++i) {
+    if (std::isnan(thresholds[i])) return fail(ctx, TPE_E_INVALID, "acquisition threshold %d is NaN", i);
+    if (i > 0 && !std::isfinite(thresholds[i]))
+      return fail(ctx, TPE_E_INVALID, "acquisition threshold %d is not finite", i);
+  }
+  if (kind == TPE_ACQF_LOGEI && std::isinf(thresholds[0]) && thresholds[0] > 0)
+    return fail(ctx, TPE_E_INVALID, "the LogEI threshold is +inf");
+  std::vector<uint64_t> gen(n_gp);
+  int32_t P = 0;
+  for (int i = 0; i < n_gp; ++i) {
+    tpe_ctx* g = gps[i];
+    if (!g || g == ctx) return fail(ctx, TPE_E_INVALID, "GP context %d is NULL or the acquisition context itself", i);
+    for (int j = 0; j < i; ++j)
+      if (gps[j] == g) return fail(ctx, TPE_E_INVALID, "GP contexts %d and %d are the same context", j, i);
+    if (g->device != ctx->device)
+      return fail(ctx, TPE_E_INVALID, "GP context %d is on device %d, the acquisition context on device %d", i,
+                  g->device, ctx->device);
+    std::lock_guard<std::mutex> gl(g->mu);
+    if (!g->gp.ready || !g->gp.conditioned)
+      return fail(ctx, TPE_E_STATE, "GP context %d is not conditioned (tpe_gp_condition)", i);
+    if (i > 0 && g->gp.P != P)
+      return fail(ctx, TPE_E_INVALID, "GP context %d has width %d, GP context 0 has width %d", i, g->gp.P, P);
+    P = g->gp.P;
+    gen[i] = g->gp_generation;
+  }
+  if (set_device(ctx)) return TPE_E_CUDA;
+  if (kind == TPE_ACQF_LOGEHVI) {
+    const int rc = ehvi_upload(ctx, lower, intervals, B, samples, S, n_obj);
+    if (rc != TPE_OK) return rc;
+  }
+  a.gps.assign(gps, gps + n_gp);
+  a.gen = gen;
+  a.ev.assign(n_gp, nullptr);
+  for (auto& e : a.ev) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
+  CU(a.thr.ensure((size_t)n_gp * 8));
+  CU(cudaMemcpyAsync(a.thr.p, thresholds, (size_t)n_gp * 8, cudaMemcpyHostToDevice, ctx->stream));
+  CU(cudaStreamSynchronize(ctx->stream));
+  a.kind = kind;
+  a.n_obj = n_obj;
+  a.P = P;
+  a.noise = stabilizing_noise;
+  a.ready = true;
+  return TPE_OK;
+}
+
+// The checks and the body of tpe_acqf_eval, called with the acquisition context and every GP context locked
+static int acqf_eval_locked(tpe_ctx* ctx, const double* X, int64_t Q, double* value, double* grad_h) {
+  AcqfState& a = ctx->acqf;
+  const int K = (int)a.gps.size(), P = a.P, M = a.n_obj;
+  for (int i = 0; i < K; ++i) {
+    const tpe_ctx* g = a.gps[i];
+    if (!g->gp.ready || !g->gp.conditioned || g->gp_generation != a.gen[i] || g->gp.P != P)
+      return fail(ctx, TPE_E_STATE, "GP context %d was re-conditioned or changed since tpe_acqf_set", i);
+  }
+  // non-finite query points are evaluated, not refused: NaN propagates through the posterior and the acquisition as
+  // in torch, so that an L-BFGS-B run that met a NaN gradient ends as the reference's does
+  const bool grad = grad_h != nullptr;
+  const bool ehvi_on = a.kind == TPE_ACQF_LOGEHVI;
+  auto more = [](const DevBuf& b, size_t bytes) { return bytes > b.cap ? bytes : (size_t)0; };
+  size_t need = more(a.X, (size_t)Q * P * 8) + more(a.mean, (size_t)K * Q * 8) + more(a.var, (size_t)K * Q * 8) +
+                more(a.value, (size_t)Q * 8);
+  if (grad)
+    need += more(a.dmean, (size_t)K * Q * P * 8) + more(a.dvar, (size_t)K * Q * P * 8) +
+            more(a.coef, (size_t)K * Q * 2 * 8) + more(a.grad, (size_t)Q * P * 8);
+  if (ehvi_on) need += ehvi_new_bytes(ctx->ehvi, Q, grad, true);
+  if (set_device(ctx)) return TPE_E_CUDA;
+  if (need > 0) {
+    size_t free_b = 0, total_b = 0;
+    CU(cudaMemGetInfo(&free_b, &total_b));
+    if (need > free_b)
+      return fail(ctx, TPE_E_INVALID,
+                  "the acquisition function at Q = %lld rows needs %zu more bytes of device memory, device %d has %zu "
+                  "free", (long long)Q, need, ctx->device, free_b);
+  }
+  cudaStream_t st = ctx->stream;
+  CU(a.X.ensure((size_t)Q * P * 8));
+  CU(a.mean.ensure((size_t)K * Q * 8));
+  CU(a.var.ensure((size_t)K * Q * 8));
+  CU(a.value.ensure((size_t)Q * 8));
+  if (grad) {
+    CU(a.dmean.ensure((size_t)K * Q * P * 8));
+    CU(a.dvar.ensure((size_t)K * Q * P * 8));
+    CU(a.coef.ensure((size_t)K * Q * 2 * 8));
+    CU(a.grad.ensure((size_t)Q * P * 8));
+  }
+  CU(cudaMemcpyAsync(a.X.p, X, (size_t)Q * P * 8, cudaMemcpyHostToDevice, st));
+  double *mean = a.mean.as<double>(), *var = a.var.as<double>();
+  for (int i = 0; i < K; ++i) {
+    // the GP's factor and scratch are written on its own stream
+    CU(cudaEventRecord(a.ev[i], a.gps[i]->stream));
+    CU(cudaStreamWaitEvent(st, a.ev[i], 0));
+    acqf_posterior(st, a.gps[i]->gp, a.X.as<double>(), Q, mean + (int64_t)i * Q, var + (int64_t)i * Q,
+                   grad ? a.dmean.as<double>() + (int64_t)i * Q * P : nullptr,
+                   grad ? a.dvar.as<double>() + (int64_t)i * Q * P : nullptr);
+  }
+  EhviState& e = ctx->ehvi;
+  if (ehvi_on) {
+    CU(e.mean.ensure((size_t)Q * M * 8));
+    CU(e.sd.ensure((size_t)Q * M * 8));
+    acqf::k_acqf_ehvi_in<<<(unsigned)((Q * M + 255) / 256), 256, 0, st>>>(mean, var, Q, M, a.noise,
+                                                                          e.mean.as<double>(), e.sd.as<double>());
+    const int rc = ehvi_launch(ctx, e.mean.as<double>(), e.sd.as<double>(), Q, grad);
+    if (rc != TPE_OK) return rc;
+  }
+  acqf::k_acqf_combine<<<(unsigned)((Q + 127) / 128), 128, 0, st>>>(
+      a.kind, K, M, a.thr.as<double>(), a.noise, mean, var, Q, ehvi_on ? e.value.as<double>() : nullptr,
+      ehvi_on && grad ? e.dmean.as<double>() : nullptr, ehvi_on && grad ? e.dsd.as<double>() : nullptr,
+      ehvi_on ? e.sd.as<double>() : nullptr, a.value.as<double>(), grad ? a.coef.as<double>() : nullptr);
+  if (grad)
+    acqf::k_acqf_grad<<<(unsigned)((Q * P + 255) / 256), 256, 0, st>>>(K, a.coef.as<double>(), a.dmean.as<double>(),
+                                                                       a.dvar.as<double>(), Q, P, a.grad.as<double>());
+  CU(cudaGetLastError());
+  CU(cudaMemcpyAsync(value, a.value.p, (size_t)Q * 8, cudaMemcpyDeviceToHost, st));
+  if (grad) CU(cudaMemcpyAsync(grad_h, a.grad.p, (size_t)Q * P * 8, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return TPE_OK;
+}
+
+// replaces eval_acqf of GPSampler's acquisition functions (acqf.py:151-159, 175-182, 237-242, 282-300, 333-337) and
+// its autograd backward in x
+int tpe_acqf_eval(tpe_ctx* ctx, const double* X, int64_t Q, double* value, double* grad) {
+  if (!ctx) return TPE_E_INVALID;
+  std::lock_guard<std::mutex> lk(ctx->mu);
+  AcqfState& a = ctx->acqf;
+  if (!a.ready) return fail(ctx, TPE_E_STATE, "no acquisition function (tpe_acqf_set)");
+  if (!X || !value || Q < 1) return fail(ctx, TPE_E_INVALID, "bad acquisition arguments (Q %lld)", (long long)Q);
+  // the GP contexts in address order, so that two acquisition contexts sharing GPs cannot deadlock
+  std::vector<tpe_ctx*> order(a.gps);
+  std::sort(order.begin(), order.end());
+  std::vector<std::unique_lock<std::mutex>> held;
+  held.reserve(order.size());
+  for (tpe_ctx* g : order) held.emplace_back(g->mu);
+  return acqf_eval_locked(ctx, X, Q, value, grad);
 }
 
 // replaces get_non_dominated_box_bounds (optuna/_hypervolume/box_decomposition.py:138-157), as LogEHVI.__init__ calls

@@ -62,6 +62,7 @@ class TPEEngine:
         self._cols: list[int] = []
         self._gp_P = 0
         self._ehvi_M = 0
+        self._acqf_P = 0
 
     # -- lifecycle -----------------------------------------------------------------------------
     def close(self) -> None:
@@ -606,6 +607,47 @@ class TPEEngine:
         dsd = np.empty(m.shape) if grad else None
         self._check(self._lib.tpe_ehvi(self._h, _ptr(m), _ptr(s), m.shape[0], _ptr(value), _ptr(dmean), _ptr(dsd)))
         return (value, dmean, dsd) if grad else value
+
+    ACQF_LOGEI, ACQF_LOGEHVI, ACQF_LOGPI = 0, 1, 2   # tpe_acqf_set's kinds
+
+    def acqf_set(self, kind: int, gp_engines, n_obj: int, thresholds, stabilizing_noise: float = 1e-12,
+                 lower=None, intervals=None, samples=None) -> None:
+        """GPSampler's acquisition function over the conditioned GPs of ``gp_engines`` (tpe_acqf_set): ``ACQF_LOGEI``
+        (``n_obj`` = 1, LogEI of the first GP), ``ACQF_LOGEHVI`` (2 <= ``n_obj`` <= 24, log-EHVI of the first
+        ``n_obj`` GPs over ``lower`` / ``intervals`` [B, M] and ``samples`` [S, M]) or ``ACQF_LOGPI`` (``n_obj`` = 0);
+        the GPs after the objectives' are constraints whose LogPI terms are added.  ``thresholds`` holds one value
+        per GP (LogEI's may be -inf).  The engines must stay open while this one evaluates; conditioning one of them
+        again invalidates the acquisition."""
+        engines = list(gp_engines)
+        thr = _f64(thresholds).reshape(-1)
+        if thr.shape != (len(engines),):
+            raise ValueError(f"one threshold per GP engine: {len(engines)} engines, {thr.size} thresholds")
+        handles = (C.c_void_p * max(len(engines), 1))(*[e._h for e in engines])
+        lb = iv = z = None
+        B = S = 0
+        if kind == self.ACQF_LOGEHVI:
+            lb, iv, z = _f64(lower), _f64(intervals), _f64(samples)
+            if lb.ndim != 2 or iv.shape != lb.shape or z.ndim != 2 or z.shape[1] != lb.shape[1]:
+                raise ValueError(f"EHVI inputs must be lower [B, M], intervals [B, M], samples [S, M]; got {lb.shape}, "
+                                 f"{iv.shape}, {z.shape}")
+            B, S = lb.shape[0], z.shape[0]
+        self._acqf_P = 0
+        self._check(self._lib.tpe_acqf_set(self._h, int(kind), handles, len(engines), int(n_obj), _ptr(thr),
+                                           float(stabilizing_noise), _ptr(lb), _ptr(iv), B, _ptr(z), S))
+        self._acqf_P = engines[0]._gp_P
+        self._acqf_engines = engines   # kept open with this acquisition
+
+    def acqf_eval(self, X, grad: bool = False):
+        """The acquisition function of ``acqf_set`` at the rows of ``X`` [Q, P] (tpe_acqf_eval): ``value`` [Q] and
+        with ``grad`` also d value / dx [Q, P], in one device call.  A row's value is the same bits whatever the batch
+        and the gradient request."""
+        x = _f64(X)
+        if x.ndim != 2 or (self._acqf_P and x.shape[1] != self._acqf_P):
+            raise ValueError(f"X must be [Q, {self._acqf_P}], got shape {x.shape}")
+        value = np.empty(x.shape[0])
+        g = np.empty(x.shape) if grad else None
+        self._check(self._lib.tpe_acqf_eval(self._h, _ptr(x), x.shape[0], _ptr(value), _ptr(g)))
+        return (value, g) if grad else value
 
     def box_decomposition(self, loss_vals, ref_point) -> tuple[np.ndarray, np.ndarray]:
         """``get_non_dominated_box_bounds(loss_vals, ref_point)`` (optuna/_hypervolume/box_decomposition.py:138-157)

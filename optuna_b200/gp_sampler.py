@@ -23,6 +23,11 @@ computes the Pareto filter and reference point before the decomposition, the QMC
 terms on the host; the other acquisition functions run unchanged over the device GPs.  Beyond 24 objectives optuna's
 host ``LogEHVI`` is kept.
 
+The acquisition search is optuna's ``optimize_acqf_mixed`` restated step for step (``_acqf_search``) over a fused
+device acquisition (``TPEEngine.acqf_set`` / ``acqf_eval``): the GPs' posteriors, LogEI / LogPI / log-EHVI and the
+gradient in x in one call, and every round of the live local searches gathered into that call.  A row's value does
+not depend on its batch, so the suggestion is the bits of optuna's own search over the same acquisition.
+
 One difference: the device holds two n x n fp64 matrices per GP and a pool of the decomposition's bounds, and
 ``sample_relative`` raises ``ValueError`` naming the need when the device lacks that memory.
 """
@@ -44,6 +49,7 @@ from optuna.samplers._gp.sampler import EPS, _get_constraint_vals_and_feasibilit
 from optuna.study import StudyDirection
 from optuna.study._multi_objective import _is_pareto_front
 
+from . import _acqf_search
 from .engine import GPCholeskyError, TPEEngine
 from .terminator import _fit
 
@@ -59,6 +65,13 @@ def _answers_ehvi(engine_cls) -> bool:
     kernel is an error.  A substitute engine that restates only the GP calls (a host implementation of them) leaves the
     acquisition to optuna's host ``LogEHVI``, as before the device log-EHVI existed."""
     return callable(getattr(engine_cls, "ehvi_set", None)) and callable(getattr(engine_cls, "ehvi", None))
+
+
+def _answers_acqf(engine_cls) -> bool:
+    """Whether ``engine_cls`` answers the fused acquisition calls (``acqf_set`` / ``acqf_eval``).  ``TPEEngine``
+    always does; with a substitute engine without them the acquisition search stays optuna's, over the per-GP
+    queries."""
+    return callable(getattr(engine_cls, "acqf_set", None)) and callable(getattr(engine_cls, "acqf_eval", None))
 
 
 def _answers_box_decomposition(engine_cls) -> bool:
@@ -171,6 +184,7 @@ class _DeviceLogEHVI(acqf_module.BaseAcquisitionFunc):
     device call."""
 
     def __init__(self, host: acqf_module.LogEHVI, engine) -> None:
+        self._host = host
         self._gpr_list = host._gpr_list
         self._stabilizing_noise = host._stabilizing_noise
         self._engine = engine
@@ -185,6 +199,79 @@ class _DeviceLogEHVI(acqf_module.BaseAcquisitionFunc):
             means.append(mean)
             sds.append(torch.sqrt(var + self._stabilizing_noise))
         return _EHVI.apply(torch.stack(means, dim=-1), torch.stack(sds, dim=-1), self._engine)
+
+
+class _AcqfValue(torch.autograd.Function):
+    """``eval_acqf`` from one ``acqf_eval``; the backward is ``g dvalue/dx`` with the gradient that call returned."""
+
+    @staticmethod
+    def forward(ctx: Any, x: torch.Tensor, acqf: _DeviceAcqf) -> torch.Tensor:
+        want_grad = ctx.needs_input_grad[0]
+        xs = x.detach().cpu().numpy().reshape(-1, x.shape[-1])
+        out = acqf.evaluate(xs, want_grad)
+        if not want_grad:
+            return torch.from_numpy(out).reshape(x.shape[:-1])
+        ctx.save_for_backward(torch.from_numpy(out[1]).reshape(x.shape))
+        return torch.from_numpy(out[0]).reshape(x.shape[:-1])
+
+    @staticmethod
+    def backward(ctx: Any, g: torch.Tensor) -> tuple[torch.Tensor, None]:
+        (dx,) = ctx.saved_tensors
+        return g[..., None] * dx, None
+
+
+class _DeviceAcqf(acqf_module.BaseAcquisitionFunc):
+    """GPSampler's acquisition function (LogEI, ConstrainedLogEI, LogEHVI, ConstrainedLogEHVI) evaluated by one
+    ``acqf_eval`` of ``engine`` per call, value and gradient, over the conditioned device GPs of the host object it
+    replaces, with that object's thresholds, stabilising noise, boxes, samples, length scales and search space.
+    ``calls`` counts the device calls."""
+
+    def __init__(self, engine, kind: int, n_obj: int, gprs: list[_DeviceGP], thresholds: list[float], noise: float,
+                 host: acqf_module.BaseAcquisitionFunc, ehvi: acqf_module.LogEHVI | None = None) -> None:
+        self._engine = engine
+        self.calls = 0
+        boxes = {} if ehvi is None else dict(lower=ehvi._non_dominated_box_lower_bounds.numpy(),
+                                             intervals=ehvi._non_dominated_box_intervals.numpy(),
+                                             samples=ehvi._fixed_samples.numpy())
+        engine.acqf_set(kind, [gpr._engine for gpr in gprs], n_obj, thresholds, noise, **boxes)
+        super().__init__(host.length_scales, host.search_space)
+
+    @classmethod
+    def build(cls, engine, acqf: acqf_module.BaseAcquisitionFunc) -> _DeviceAcqf | None:
+        """The device form of the acquisition function ``GPSampler`` built, or None when it has none: optuna's host
+        ``LogEHVI`` (beyond 24 objectives, or an engine class without the log-EHVI calls) stays on optuna's path."""
+        cons: list = []
+        ehvi = None
+        if type(acqf) is acqf_module.LogEI:
+            kind, objs, thr = TPEEngine.ACQF_LOGEI, [acqf], [acqf._threshold]
+        elif type(acqf) is acqf_module.ConstrainedLogEI:
+            kind, objs, thr = TPEEngine.ACQF_LOGEI, [acqf._acqf], [acqf._acqf._threshold]
+            cons = acqf._constraints_acqf_list
+        elif type(acqf) is _DeviceLogEHVI:
+            kind, objs, thr, ehvi = TPEEngine.ACQF_LOGEHVI, [acqf], [], acqf._host
+        elif type(acqf) is acqf_module.ConstrainedLogEHVI and acqf._acqf is None:
+            kind, objs, thr = TPEEngine.ACQF_LOGPI, [], []
+            cons = acqf._constraints_acqf_list
+        elif type(acqf) is acqf_module.ConstrainedLogEHVI and type(acqf._acqf) is _DeviceLogEHVI:
+            kind, objs, thr, ehvi = TPEEngine.ACQF_LOGEHVI, [acqf._acqf], [], acqf._acqf._host
+            cons = acqf._constraints_acqf_list
+        else:
+            return None
+        gprs = [o._gpr for o in objs if hasattr(o, "_gpr")] + [g for o in objs for g in getattr(o, "_gpr_list", [])]
+        gprs += [c._gpr for c in cons]
+        thr = thr + [0.0] * (len(gprs) - len(cons) - len(thr)) + [c._threshold for c in cons]
+        noises = {o._stabilizing_noise for o in objs + cons}
+        if len(noises) != 1 or not all(isinstance(g, _DeviceGP) for g in gprs):
+            return None
+        n_obj = len(gprs) - len(cons)
+        return cls(engine, kind, n_obj, gprs, [float(t) for t in thr], noises.pop(), acqf, ehvi)
+
+    def evaluate(self, x: np.ndarray, grad: bool):
+        self.calls += 1
+        return self._engine.acqf_eval(x, grad=grad)
+
+    def eval_acqf(self, x: torch.Tensor) -> torch.Tensor:
+        return _AcqfValue.apply(x, self)
 
 
 class GPSampler(_OptunaGPSampler):
@@ -225,6 +312,7 @@ class GPSampler(_OptunaGPSampler):
         self._device = device
         self._engines: list = []   # one per GP: the objectives', then the constraints'
         self._ehvi_engine = None   # the log-EHVI acquisition's, created on the first multi-objective ask
+        self._acqf_engine = None   # the fused acquisition's (acqf_set / acqf_eval), created on the first search
         # study.optimize(n_jobs > 1) samples on several threads, and a trial's fits, conditioning and queries on the
         # shared engines must not interleave with another trial's
         self._lock = threading.RLock()
@@ -237,6 +325,9 @@ class GPSampler(_OptunaGPSampler):
             if self._ehvi_engine is not None:
                 self._ehvi_engine.close()
                 self._ehvi_engine = None
+            if self._acqf_engine is not None:
+                self._acqf_engine.close()
+                self._acqf_engine = None
 
     def __del__(self) -> None:  # pragma: no cover
         try:
@@ -295,6 +386,27 @@ class GPSampler(_OptunaGPSampler):
         acqf_module.BaseAcquisitionFunc.__init__(host, np.mean([gpr.length_scales for gpr in gpr_list], axis=0),
                                                  search_space)
         return self._device_ehvi(host)
+
+    def _optimize_acqf(self, acqf: acqf_module.BaseAcquisitionFunc, best_params: np.ndarray | None) -> np.ndarray:
+        """optuna's ``_optimize_acqf`` (optuna/samplers/_gp/sampler.py:237-252).  When the engine class answers the
+        fused acquisition calls (``_answers_acqf``), ``optimize_acqf_mixed`` runs as ``_acqf_search`` restates it
+        over the device acquisition (``_DeviceAcqf``): every round of the live local searches is one device call, and
+        the suggestion is the bits optuna's own search over that acquisition returns.  Otherwise, and for optuna's
+        host ``LogEHVI``, optuna's search runs unchanged."""
+        device = None
+        if _answers_acqf(_engine_cls):
+            if self._acqf_engine is None:
+                self._acqf_engine = _engine_cls(self._device)
+            device = _DeviceAcqf.build(self._acqf_engine, acqf)
+        if device is None:
+            return super()._optimize_acqf(acqf, best_params)
+        assert best_params is None or len(best_params.shape) == 2
+        normalized_params, _acqf_val = _acqf_search.optimize_acqf_mixed(
+            device, device.evaluate, warmstart_normalized_params_array=best_params,
+            n_preliminary_samples=self._n_preliminary_samples, n_local_search=self._n_local_search, tol=self._tol,
+            rng=self._rng.rng)
+        self.last_acqf_calls = device.calls
+        return normalized_params
 
     def _get_constraints_acqf_args(self, constraint_vals: np.ndarray,
                                    internal_search_space: gp_search_space.SearchSpace,

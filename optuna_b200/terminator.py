@@ -347,32 +347,30 @@ class _Prefix:
 
 
 class _LockStep:
-    """Lock-step L-BFGS-B: one scipy fit thread per task.  A thread's loss call posts the GP it fits and its raw
-    parameters and blocks; ``run`` evaluates everything posted in one ``gp_batch_loss``, then releases the threads one
-    at a time and waits for each to post again or finish.  So one fit thread runs at a time (the host work is serial
-    under the GIL anyway) and the threads do not contend for the GIL; a thread whose task has returned leaves the
-    batch.  With ``deterministic`` every fit holds the noise at ``minimum_noise`` (the fixed-noise batched loss)."""
+    """Lock-step evaluation for one thread per task (scipy's L-BFGS-B or Brent searches).  A thread's ``post`` hands
+    over its payload and blocks; ``run`` evaluates everything posted in one ``evaluate(payloads)`` call (the payloads
+    in key order, one result each), then releases the threads one at a time and waits for each to post again or
+    finish.  So one thread runs at a time (the host work is serial under the GIL anyway) and the threads do not
+    contend for the GIL; a thread that calls ``leave`` drops out of the batch."""
 
-    def __init__(self, engine, minimum_noise: float, deterministic: bool = False) -> None:
-        self._engine = engine
-        self._minimum_noise = minimum_noise
-        self.deterministic = deterministic
+    def __init__(self, evaluate) -> None:
+        self._evaluate = evaluate
         self._cond = threading.Condition()
-        self._posted: dict[int, tuple[int, np.ndarray]] = {}
+        self._posted: dict[int, object] = {}
         self._left: set[int] = set()
-        self._results: dict[int, tuple] = {}
+        self._results: dict[int, object] = {}
         self._events: dict[int, threading.Event] = {}
         self.rounds = 0
         self.device_seconds = 0.0
 
-    def slot(self, key: int) -> "_Slot":
+    def join(self, key: int) -> None:
+        """Registers the thread of ``key`` before it starts."""
         self._events[key] = threading.Event()
-        return _Slot(self, key)
 
-    def post(self, key: int, gp: int, raw: np.ndarray):
+    def post(self, key: int, payload):
         ev = self._events[key]
         with self._cond:
-            self._posted[key] = (gp, raw)
+            self._posted[key] = payload
             self._cond.notify()
         ev.wait()
         ev.clear()
@@ -389,6 +387,7 @@ class _LockStep:
                 self._cond.wait()
 
     def run(self, threads: list) -> None:
+        """Starts ``threads[k]`` (the thread of key k) and serves their posts until every one has left."""
         import time
         for key, th in enumerate(threads):
             th.start()
@@ -396,34 +395,44 @@ class _LockStep:
         while self._posted:
             batch, self._posted = self._posted, {}
             keys = sorted(batch)
-            gps = [batch[k][0] for k in keys]
-            raws = np.stack([batch[k][1] for k in keys])
             t0 = time.perf_counter()
-            if self.deterministic:
-                loss, grad, status = self._engine.gp_batch_loss(gps, raws, self._minimum_noise, deterministic=True)
-            else:
-                loss, grad, status = self._engine.gp_batch_loss(gps, raws, self._minimum_noise)
+            results = self._evaluate([batch[k] for k in keys])
             self.device_seconds += time.perf_counter() - t0
             self.rounds += 1
-            for i, k in enumerate(keys):
-                self._results[k] = (float(loss[i]), grad[i].copy(), int(status[i]))
+            for k, r in zip(keys, results):
+                self._results[k] = r
                 self._events[k].set()
                 self._wait(k)
+
+
+def _batch_loss(engine, minimum_noise: float, deterministic: bool):
+    """The lock-step evaluation of the batched fits: one ``gp_batch_loss`` over the posted (GP, raw parameters)."""
+    def evaluate(posted: list) -> list:
+        gps = [gp for gp, _ in posted]
+        raws = np.stack([raw for _, raw in posted])
+        if deterministic:
+            loss, grad, status = engine.gp_batch_loss(gps, raws, minimum_noise, deterministic=True)
+        else:
+            loss, grad, status = engine.gp_batch_loss(gps, raws, minimum_noise)
+        return [(float(loss[i]), grad[i].copy(), int(status[i])) for i in range(len(posted))]
+    return evaluate
 
 
 class _Slot:
     """The engine a fit thread sees: ``gp_loss`` answered by the lock-step batch, for the GP ``gp`` of the wave
     (the thread's own index unless its task sets another)."""
 
-    def __init__(self, lockstep: _LockStep, key: int) -> None:
+    def __init__(self, lockstep: _LockStep, key: int, deterministic: bool) -> None:
         self._ls = lockstep
         self._key = key
+        self._deterministic = deterministic
         self.gp = key
+        lockstep.join(key)
 
     def gp_loss(self, raw_params, minimum_noise: float, deterministic: bool = False):
-        if deterministic != self._ls.deterministic:
+        if deterministic != self._deterministic:
             raise ValueError("a fit's noise model differs from its lock-step batch's")
-        loss, grad, status = self._ls.post(self._key, self.gp, np.array(raw_params, dtype=np.float64))
+        loss, grad, status = self._ls.post(self._key, (self.gp, np.array(raw_params, dtype=np.float64)))
         if status:
             raise GPCholeskyError("the GP covariance is not positive definite")
         return loss, grad
@@ -469,7 +478,7 @@ def _fit_wave(engine, data: list[tuple[np.ndarray, np.ndarray]], is_categorical,
     offsets[1:] = np.cumsum([X.shape[0] for X, _ in data])
     engine.gp_batch_set(offsets, np.concatenate([X for X, _ in data]), np.concatenate([y for _, y in data]),
                         is_categorical)
-    ls = _LockStep(engine, minimum_noise, deterministic)
+    ls = _LockStep(_batch_loss(engine, minimum_noise, deterministic))
     results: dict[int, object] = {}
     errors: dict[int, BaseException] = {}
 
@@ -481,7 +490,8 @@ def _fit_wave(engine, data: list[tuple[np.ndarray, np.ndarray]], is_categorical,
         finally:
             ls.leave(k)
 
-    threads = [threading.Thread(target=work, args=(k, ls.slot(k)), daemon=True) for k in range(len(tasks))]
+    threads = [threading.Thread(target=work, args=(k, _Slot(ls, k, deterministic)), daemon=True)
+               for k in range(len(tasks))]
     ls.run(threads)
     for th in threads:
         th.join()
